@@ -68,11 +68,12 @@ def load_peaks():
         # the conv / RVQ kernels are timed inside a long step: the SUSTAINED dense bf16 figure is the tensor denominator
         return dict(hbm_gbs=float(d["hbm_gbs"]), bf16_tflops=float(d.get("bf16_tflops_sustained", d.get("bf16_tflops", 0))),
                     source="measured")
-    return dict(hbm_gbs=6650.0, bf16_tflops=1590.0, source="fallback")
+    # NVIDIA H100 SXM data sheet (700 W card): 3.35 TB/s HBM3, 989 TFLOP/s dense BF16
+    return dict(hbm_gbs=3350.0, bf16_tflops=989.0, source="H100 SXM data sheet")
 
 
 class ClockSampler:
-    """nvidia-smi clocks / throttle reasons sampled during the timed region (B200_PROFILING.md recipe)."""
+    """nvidia-smi clocks / throttle reasons sampled during the timed region (read-only queries)."""
 
     def __init__(self, index):
         self.index = index
@@ -321,6 +322,28 @@ def config5_extra(model, cfg, dev, rank, world, steps=5):
     return out
 
 
+DUMP_BUDGET = 60_000_000        # bytes --dump-outputs may write in all, .npy headers included (under 64 MB either way)
+NPY_HEADER = 4096               # generous bound on one .npy header
+
+
+def dump_outputs(out_dir, arrays):
+    """Writes what the timed path returned in its last step as DIR/<name>.npy (float32).  An array larger than its share of
+    the budget is replaced by a fixed, seeded sample of its flattened elements (`<name>.npy`) plus the flat indices of that
+    sample (`<name>_index.npy`, float64), so two builds can be compared element for element."""
+    import numpy as np
+    os.makedirs(out_dir, exist_ok=True)
+    share = DUMP_BUDGET // len(arrays)
+    for name, t in arrays.items():
+        a = t.detach().float().cpu().numpy().ravel()
+        if a.nbytes + NPY_HEADER <= share:
+            np.save(os.path.join(out_dir, f"{name}.npy"), t.detach().float().cpu().numpy())
+            continue
+        n = (share - 2 * NPY_HEADER) // 12                 # float32 value + float64 index per sampled element
+        idx = np.sort(np.random.default_rng(0).choice(a.size, size=n, replace=False))
+        np.save(os.path.join(out_dir, f"{name}.npy"), a[idx])
+        np.save(os.path.join(out_dir, f"{name}_index.npy"), idx.astype(np.float64))
+
+
 def cuda_eager_reference(cfg, sd, B, L, dev, reps=3):
     """Context only (BASELINE.md 'secondary comparison'): the oracle's torch functional restatement of the reference modules
     run on the SAME GPU in eager mode with TF32 off (cuDNN / cuBLAS fp32 kernels), device-resident input."""
@@ -349,6 +372,10 @@ def main():
     ap.add_argument("--steps", type=int, default=10)
     ap.add_argument("--warmup", type=int, default=3)
     ap.add_argument("--impl", default="b200", choices=["b200", "reference"])
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="after the timed steps, write the last step's outputs (codes, quantized embeddings, scale, "
+                         "reconstruction) as DIR/<name>.npy in float32, at most 60 MB in all; an output larger than its "
+                         "share is written as a seeded sample plus its flat indices (DIR/<name>_index.npy)")
     ap.add_argument("--workload", default="config2", choices=sorted(WORKLOADS))
     ap.add_argument("--batch", type=int, default=0, help="override per-GPU batch")
     ap.add_argument("--no-cpu-baseline", action="store_true")
@@ -360,6 +387,8 @@ def main():
     args = ap.parse_args()
     args.warmup = max(args.warmup, 3) if args.impl == "b200" else args.warmup
     if args.impl == "reference":
+        if args.dump_outputs:
+            ap.error("--dump-outputs dumps the CUDA path's outputs; it is not available with --impl reference")
         return run_reference(args)
 
     import torch
@@ -444,6 +473,8 @@ def main():
     e1.record()
     barrier()
     ms = e0.elapsed_time(e1)
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, dict(codes=codes, quant=quant, scale=scale, recon=recon))
     launches = model.launch_count() - launches0
     phases = model.phase_ms()           # the last timed step's phase durations
     model.set_profiling(False)
@@ -547,16 +578,16 @@ def main():
         conv_tflops = 2 * algo["conv_gmac_per_10s"] * clip10 * B / (conv_ms * 1e-3) / 1e3 if conv_ms > 0 else 0.0
         traffic, traffic_src = load_ncu_traffic(args.workload) if not args.batch else (None, None)
         # tensor-pipe view (north_star: "tensor-pipe utilisation (RVQ distance)"): fp32-equivalent FLOPs x 3 passes of the split
-        # operands, against the measured dense bf16/fp16 rate (conv: kind::f16) or half of it (RVQ: kind::tf32)
+        # operands, against the dense bf16/fp16 rate (conv: fp16 wgmma) or half of it (RVQ: tf32 wgmma)
         f16_peak = peaks["bf16_tflops"]
         conv_tensor_tflops = 3 * conv_tflops
         rvq_ms = phases.get("rvq", 0.0)
         rvq_tflops = 3 * algo["rvq_gflop_per_10s_nq32"] * (n_q / 32.0) * clip10 * B / (rvq_ms * 1e-3) / 1e3 if rvq_ms > 0 else 0.0
         tensor = dict(conv=dict(achieved=conv_tensor_tflops, peak=f16_peak, unit="TFLOP/s", frac=conv_tensor_tflops / f16_peak if f16_peak else None,
-                                note="3 kind::f16 MMAs per fp32-equivalent product (fp16 hi/lo split); peak = measured dense bf16"),
+                                note="3 fp16 wgmma per fp32-equivalent product (fp16 hi/lo split); peak = dense bf16 (measured, else data sheet)"),
                       rvq=dict(achieved=rvq_tflops, peak=f16_peak / 2, unit="TFLOP/s", frac=rvq_tflops / (f16_peak / 2) if f16_peak else None,
                                kernel_ms_per_step=rvq_ms,
-                               note="rvq_tc_kernel: 3 kind::tf32 MMAs per product; peak = measured dense bf16 / 2 (tf32 rate); "
+                               note="rvq_tc_kernel: 3 tf32 wgmma per product; peak = dense bf16 / 2 (tf32 rate); "
                                     "includes the argmin / re-scoring / residual-update epilogues of all stages"))
         roofline = dict(bound="hbm", kernel="conv1d_tc_kernel<N> (+ conv1d_cl / conv1d_cout1 for the 3 layers that do not fit "
                                             "the tensor cores): all SEANet conv/convtr launches of one step = "
@@ -578,7 +609,7 @@ def main():
                     rtf=(ms_max * 1e-3) / audio_s,
                     config=dict(workload=f"{cfg_name} B={B}/GPU L={L} n_q={n_q} (BASELINE {args.workload})",
                                 global_batch=world * B, clip_seconds=L / cfg.sample_rate,
-                                l2="inputs rotated over %d distinct batches (>126 MB); per-step activation traffic >> L2" % n_rot,
+                                l2="inputs rotated over %d distinct batches (>140 MB); per-step activation traffic >> L2" % n_rot,
                                 parallelism=f"dp{world} (independent clips per GPU)"),
                     clocks=clocks, gpu_launches=int(launches),
                     e2e=dict(value=e2e_value, unit="frames/s", h2d_bytes_per_step=int(h2d), d2h_bytes_per_step=int(d2h),

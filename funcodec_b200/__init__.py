@@ -1,4 +1,4 @@
-"""funcodec_b200: B200-native (sm_100a) codec encode -> RVQ -> decode hot path for FunCodec."""
+"""funcodec_b200: H100-native (sm_90a) codec encode -> RVQ -> decode hot path for FunCodec."""
 from .config import CodecConfig, PRESETS, get_config  # noqa: F401
 from .weights import init_state_dict, state_dict_shapes, conv_specs  # noqa: F401
 

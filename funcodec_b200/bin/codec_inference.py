@@ -118,7 +118,7 @@ def config_from_yaml(path: str):
 
 def get_parser():
     """Same flags, types and defaults as the reference's get_parser (codec_inference.py:428-558)."""
-    p = argparse.ArgumentParser(description="Speech Tokenizer (B200)", formatter_class=argparse.ArgumentDefaultsHelpFormatter)
+    p = argparse.ArgumentParser(description="Speech Tokenizer (H100)", formatter_class=argparse.ArgumentDefaultsHelpFormatter)
     p.add_argument("--log_level", type=lambda x: x.upper(), default="INFO",
                    choices=("CRITICAL", "ERROR", "WARNING", "INFO", "DEBUG", "NOTSET"))
     p.add_argument("--output_dir", type=str, required=False)

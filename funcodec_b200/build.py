@@ -1,4 +1,4 @@
-"""Build the C-ABI shared library (funcodec_b200/lib/libfuncodec_b200.so) with nvcc for sm_100a.
+"""Build the C-ABI shared library (funcodec_b200/lib/libfuncodec_b200.so) with nvcc for sm_90a.
 
 The library is built IN-TREE so that it travels to the GPU box with the repo snapshot.
 Usage: python -m funcodec_b200.build [--force]
@@ -13,7 +13,7 @@ CSRC = os.path.join(HERE, "csrc")
 LIBDIR = os.path.join(HERE, "lib")
 LIB = os.path.join(LIBDIR, "libfuncodec_b200.so")
 SOURCES = ["engine.cu", "conv_simt.cu", "conv_tc.cu", "conv2d_simt.cu", "lstm.cu", "rvq_simt.cu", "rvq_tc.cu", "misc.cu"]
-NVCC_FLAGS = ["-gencode", "arch=compute_100a,code=sm_100a", "-O3", "-lineinfo", "-std=c++17",
+NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17",
               "-Xcompiler", "-fPIC", "-Xcompiler", "-fvisibility=hidden", "--expt-relaxed-constexpr"]
 
 
@@ -56,7 +56,7 @@ def build(force: bool = False, verbose: bool = False) -> str:
             sys.stderr.write(out)
         if p.returncode != 0:
             raise RuntimeError(f"nvcc failed on {src}")
-    cmd = [nvcc, "-shared", "-o", LIB] + objs + ["-gencode", "arch=compute_100a,code=sm_100a", "-lcudart"]
+    cmd = [nvcc, "-shared", "-o", LIB] + objs + ["-gencode", "arch=compute_90a,code=sm_90a", "-lcudart"]
     subprocess.check_call(cmd)
     with open(stamp, "w") as f:
         f.write(dig)

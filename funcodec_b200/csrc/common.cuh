@@ -1,4 +1,4 @@
-// Shared device/host definitions for the funcodec_b200 kernels (sm_100a).
+// Shared device/host definitions for the funcodec_b200 kernels (sm_90a).
 //
 // HBM layout (DESIGN.md section 3): every activation is stored CHANNELS-LAST, [B][T][C] fp32, RAW
 // (= conv output incl. bias, before GroupNorm).  GroupNorm(1,C) needs the statistics of the whole

@@ -149,7 +149,7 @@ static void conv2d_pick(const Conv2dParams& p, int* tx, int* tm) {
     *tm = 8;
     const int CO_TILE = *tx * 8, T_TILE = (256 / *tx) * 8;
     const long long ctas = (long long)((p.T_out + T_TILE - 1) / T_TILE) * ((p.C_out_eff + CO_TILE - 1) / CO_TILE) * p.B * p.F_out;
-    if (ctas < 2 * 148) *tm = 4;
+    if (ctas < 2 * 132) *tm = 4;
 }
 
 int conv2d_num_parts(const Conv2dParams& p) {

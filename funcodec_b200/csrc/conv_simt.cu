@@ -411,10 +411,10 @@ void conv_pick_tile(int T_out, int C_out, int C_in, int K, int B, int* tx, int* 
     *tx = C_out >= 128 ? 16 : (C_out >= 64 ? 8 : (C_out >= 32 ? 4 : 2));
     *two = (long long)C_in * K >= 1024;
     *tm = 8;
-    // small problems: halve the time tile so that the grid covers the 148 SMs
+    // small problems: halve the time tile so that the grid covers the 132 SMs
     const int CO_TILE = *tx * 8, T_TILE = (256 / *tx) * 8;
     const long long ctas = (long long)((T_out + T_TILE - 1) / T_TILE) * ((C_out + CO_TILE - 1) / CO_TILE) * B;
-    if (ctas < 2 * 148) *tm = 4;
+    if (ctas < 2 * 132) *tm = 4;
 }
 
 cudaError_t launch_conv(const ConvParams& p, int B, cudaStream_t st, int* nparts) {

@@ -1,9 +1,9 @@
-// Implicit-GEMM Conv1d on the 5th-generation tensor cores (tcgen05.mma kind::f16, accumulators in TMEM),
-// fp32-faithful through a 3-term FP16 split: both operands are pre-scaled by a power of two (activations x16, weights
+// Implicit-GEMM Conv1d on the Hopper tensor cores (wgmma m64nNk16, fp16 operands in shared memory, fp32 accumulators in
+// registers), fp32-faithful through a 3-term FP16 split: both operands are pre-scaled by a power of two (activations x16, weights
 // per layer so that max|w| lands in [2^13, 2^14)), x = hi + lo with hi = fp16(x), lo = fp16(x - hi), and
-// D += lo*hi + hi*lo + hi*hi in fp32; the epilogue multiplies by the (exact) inverse scale.  Same accuracy as the
-// 3xTF32 split it replaces (both drop the lo*lo term, ~2^-22 relative), at twice the tensor throughput and half the
-// shared-memory operand bytes per MAC (K = 16 per MMA instead of 8; a 128-byte swizzle row holds 64 channels).
+// D += lo*hi + hi*lo + hi*hi in fp32; the epilogue multiplies by the (exact) inverse scale.  Same accuracy as a 3xTF32 split
+// (both drop the lo*lo term, ~2^-22 relative), at twice the tensor throughput and half the shared-memory operand bytes per
+// MAC (K = 16 per MMA instead of 8; a 128-byte swizzle row holds 64 channels).
 //
 // Same contract as conv_simt.cu (fused [GroupNorm apply + resblock add + ELU + reflect pad] on the input,
 // bias + raw store + GroupNorm partial statistics on the output), reference semantics
@@ -21,14 +21,13 @@
 //     (TMA engine, 1-D) per (chunk, tap) into a ring, completion on an mbarrier.
 //   * PERSISTENT CTAs (one per SM) walk a static list of (clip, n-tile, time-tile) tiles; every role keeps
 //     running across tile boundaries, so the next tile's loads overlap the previous tile's MMAs and epilogue.
-//   * warp roles (22 warps): 0-7 / 8-15 two producer groups taking alternate units (two units of global
-//     loads in flight; the transform is issue-bound, hence 16 warps); 16 weight copies + TMEM alloc; 17 MMA
-//     issuer; 18-21 accumulator warps.
-//   * the tensor core adds into its fp32 accumulator with truncation, so a TMEM-resident chain loses
-//     ~1 ulp per MMA (measured 5e-5 relative after 384 chained MMAs): chains are cut every ~48 MMAs, the MMA
-//     warp ping-pongs between two TMEM accumulators and the accumulator warps fold each finished group into
-//     a third TMEM region (running totals) with round-to-nearest CUDA-core adds, then run the epilogue
-//     (bias, channels-last store, GroupNorm partial sums) on the last group.
+//   * warp roles (28 warps): 0-7 / 8-15 two producer groups taking alternate units (two units of global
+//     loads in flight; the transform is issue-bound, hence 16 warps); 16 weight copies; 17 raw-tile TMA loads;
+//     20-23 / 24-27 two consumer warpgroups, each issuing the wgmma of 64 of the 128 tile rows (its A view starts
+//     64 rows further into the stage) and running the epilogue of its rows.
+//   * the tensor core adds into its fp32 accumulator with truncation, so a long chain loses ~1 ulp per MMA:
+//     chains are cut every ~48 MMAs and each finished group is folded into running totals (registers) with
+//     round-to-nearest CUDA-core adds; the epilogue (bias, channels-last store, GroupNorm partial sums) reads the totals.
 // Roofline: tensor pipe (3 MMAs per fp32-equivalent product) for the deep layers; HBM for the C <= 64 layers.
 //
 // FREQ = true is the FreqCodec 2-D mode (SConv2d / SConvTranspose2d, conv.py:317-447): a "clip" of the tile list is a
@@ -40,7 +39,7 @@
 #include <cuda.h>
 #include "common.cuh"
 #include "kernels.h"
-#include "tc_sm100.cuh"
+#include "tc_sm90.cuh"
 #include <stdlib.h>
 
 namespace fcb {
@@ -49,10 +48,11 @@ using namespace tc;
 
 constexpr int TC_M = 128;          // time rows per tile
 constexpr int TC_KC = 32;          // channels per producer unit (half of a 128-byte fp16 swizzle row)
-constexpr int TC_THREADS = 736;    // 16 producer warps (2 groups), copy warp, MMA warp, 4 accumulator warps, raw-tile TMA warp
+constexpr int TC_THREADS = 896;    // 16 producer warps (2 groups), copy warp, raw-tile TMA warp, 2 idle, 2 consumer warpgroups
+constexpr int TC_CONS_WARP0 = 20;  // first warp of the consumer warpgroups (warpgroup aligned)
 constexpr int TC_RAW_MAX = 8;      // raw activation ring (TMA-staged units): at most 8 slots
 constexpr int TC_PROD = 256;       // producer threads per group (one unit)
-constexpr int TC_GROUP_MMAS = 48;  // target number of tcgen05.mma chained in TMEM before the fp32 fold
+constexpr int TC_GROUP_MMAS = 48;  // target number of wgmma chained in one accumulator before the fp32 fold
 
 // ELU with the hardware exponential (ex2.approx): |error| <= ~2e-7 on the (0, 1] range of exp(x), the same order as
 // one fp32 rounding of the reference's exp(x) - 1.  (The SIMT path keeps expf.)
@@ -67,7 +67,7 @@ struct TcSmemLayout {
     int b_stage;       // bytes per B stage (hi + lo)
     int na, nb;        // ring depths
     int nraw, raw_slot, raw_in1, raw_cf;   // raw activation ring: slots, bytes per slot, offsets of in1 / coefficients in a slot
-    int off_b, off_stg, off_raw, off_bar, total;
+    int off_b, off_raw, off_bar, total;
 };
 
 __host__ __device__ inline TcSmemLayout tc_layout(int K, int S, int n_tile, int na, int nb, int nraw = 0, int raw_pitch = 128,
@@ -79,19 +79,18 @@ __host__ __device__ inline TcSmemLayout tc_layout(int K, int S, int n_tile, int 
     L.b_stage = 2 * n_tile * 128;
     L.na = na; L.nb = nb;
     L.off_b = na * L.a_stage;
-    L.off_stg = L.off_b + nb * L.b_stage;                  // epilogue staging: 4 warps x (32 rows x 128 B), swizzled
     // raw slot: [in0 rows][in1 rows][a0 | b0 | a1 | b1 coefficient slices of the unit's 32 channels (4 x 128 B)]
     L.nraw = nraw;
     L.raw_in1 = L.a_rows * raw_pitch;
     L.raw_cf = (1 + has1) * L.a_rows * raw_pitch;
     L.raw_slot = (L.raw_cf + 512 + 127) / 128 * 128;
-    L.off_raw = L.off_stg + 4 * 4096;
+    L.off_raw = L.off_b + nb * L.b_stage;
     L.off_bar = L.off_raw + nraw * L.raw_slot;
-    L.total = L.off_bar + 8 * (2 * na + 2 * nb + 16 + 2 * TC_RAW_MAX) + 96;
+    L.total = L.off_bar + 8 * (2 * na + 2 * nb + 2 * TC_RAW_MAX) + 160;   // + statistics scratch
     return L;
 }
 
-// ring stages (64-channel chunk, phase) chained in one TMEM accumulation group
+// ring stages (64-channel chunk, phase) chained in one accumulation group
 __host__ __device__ inline int tc_units_per_group(int K, int S, int group_mmas) {
     const int taps = (K + S - 1) / S;                  // max taps of a phase
     int g = group_mmas / (12 * taps);
@@ -103,7 +102,7 @@ __host__ __device__ inline int tc_units_per_group(int K, int S, int group_mmas) 
 struct TcArgs {
     TcSmemLayout L;
     int na, nb, n_tiles, w_resident, nraw;
-    int n_chunks, n_sc, split, n_units, upg, n_groups, n_tt, n_nt, units_per_tile, tq_rows, n_acc, raw_pitch;
+    int n_chunks, n_sc, split, n_units, upg, n_groups, n_tt, n_nt, units_per_tile, tq_rows, raw_pitch;
 };
 
 struct TcTile { int b, nt, tt; };
@@ -121,9 +120,6 @@ template <int N_TILE, bool FREQ>
 __global__ void __launch_bounds__(TC_THREADS, 1) conv1d_tc_kernel(const __grid_constant__ ConvParams p, const __grid_constant__ TcArgs ka,
                                                                  const __grid_constant__ CUtensorMap tm0,
                                                                  const __grid_constant__ CUtensorMap tm1) {
-    constexpr int BUF_COLS = N_TILE < 32 ? 32 : N_TILE;          // TMEM columns per accumulator region
-    constexpr uint32_t TMEM_COLS = 512;                          // the whole TMEM: one CTA per SM
-    constexpr int ACC_MAX = 8;                                   // accumulator ring: up to 8 tiles between MMA issue and epilogue
     extern __shared__ __align__(1024) uint8_t smem_raw[];
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
     const int C_in = p.C_in, K = p.K, S = p.S;
@@ -147,15 +143,13 @@ __global__ void __launch_bounds__(TC_THREADS, 1) conv1d_tc_kernel(const __grid_c
     uint8_t* smA = smem_raw;
     uint8_t* smB = smem_raw + L.off_b;
     uint64_t* bars = reinterpret_cast<uint64_t*>(smem_raw + L.off_bar);
-    uint64_t* a_full = bars;                       // [na]   128 producer arrivals (one group)
-    uint64_t* a_empty = a_full + na_stages;        // [na]   tcgen05.commit
+    uint64_t* a_full = bars;                       // [na]   producer arrivals (256 per group that fills the stage)
+    uint64_t* a_empty = a_full + na_stages;        // [na]   one arrival per consumer warpgroup (its wgmma have read the stage)
     uint64_t* b_full = a_empty + na_stages;        // [nb]   expect_tx
-    uint64_t* b_empty = b_full + nb_stages;        // [nb]   tcgen05.commit
-    uint64_t* acc_full = b_empty + nb_stages;      // [ACC_MAX] tcgen05.commit
-    uint64_t* acc_empty = acc_full + ACC_MAX;      // [ACC_MAX] 128 accumulator-warp arrivals
-    uint64_t* raw_full = acc_empty + ACC_MAX;      // [TC_RAW_MAX] expect_tx (TMA tile + coefficient slices)
+    uint64_t* b_empty = b_full + nb_stages;        // [nb]   one arrival per consumer warpgroup
+    uint64_t* raw_full = b_empty + nb_stages;      // [TC_RAW_MAX] expect_tx (TMA tile + coefficient slices)
     uint64_t* raw_empty = raw_full + TC_RAW_MAX;   // [TC_RAW_MAX] 256 arrivals of the consuming producer group
-    uint32_t* tmem_ptr = reinterpret_cast<uint32_t*>(raw_empty + TC_RAW_MAX);
+    double* red = reinterpret_cast<double*>(raw_empty + TC_RAW_MAX);   // [8][2] statistics scratch + finalisation flag
     uint8_t* smR = smem_raw + L.off_raw;
     // TMA-staged units (nraw > 0, 1-D layers): an INTERIOR tile needs only rows inside [0, rows covered by the tensor map) -- no
     // reflection, no zero padding -- so its units arrive as dense [a_rows][32 channel] boxes through the raw ring; the first / last
@@ -172,24 +166,14 @@ __global__ void __launch_bounds__(TC_THREADS, 1) conv1d_tc_kernel(const __grid_c
         const int hi = t_last * S - p.pad_l + (K - 1);
         return lo >= 0 && hi < tq_rows * S;
     };
-    // accumulator ring depth.  The MMA -> commit -> epilogue -> release hand-off costs ~2000 cycles per tile pair (measured: the
-    // pure barrier skeleton of the small-tile layers), so layers whose tile is one accumulation group keep up to 8 tiles in
-    // flight; layers that fold groups (deep K) ping-pong between up to 3 accumulators next to the running totals.
-#define n_acc ka.n_acc
-    double* red = reinterpret_cast<double*>(tmem_ptr + 2);       // [4][2] statistics scratch
 
     if (tid == 0) {
-        for (int i = 0; i < na_stages; ++i) { mbar_init(a_full + i, split ? 2 * TC_PROD : TC_PROD); mbar_init(a_empty + i, 1); }
-        for (int i = 0; i < nb_stages; ++i) { mbar_init(b_full + i, 1); mbar_init(b_empty + i, 1); }
-        for (int i = 0; i < ACC_MAX; ++i) { mbar_init(acc_full + i, 1); mbar_init(acc_empty + i, 128); }
+        for (int i = 0; i < na_stages; ++i) { mbar_init(a_full + i, split ? 2 * TC_PROD : TC_PROD); mbar_init(a_empty + i, 2); }
+        for (int i = 0; i < nb_stages; ++i) { mbar_init(b_full + i, 1); mbar_init(b_empty + i, 2); }
         for (int i = 0; i < TC_RAW_MAX; ++i) { mbar_init(raw_full + i, 1); mbar_init(raw_empty + i, TC_PROD); }
         mbar_fence_init();
     }
-    if (warp == 16) tmem_alloc(tmem_ptr, TMEM_COLS);
-    tc_fence_before_sync();
     __syncthreads();
-    tc_fence_after_sync();
-    const uint32_t tmem_base = *tmem_ptr;
 
     if (warp < 16) {
         // =========================================================== producers: transformed A slabs
@@ -416,65 +400,6 @@ __global__ void __launch_bounds__(TC_THREADS, 1) conv1d_tc_kernel(const __grid_c
             }
         }
     } else if (warp == 17) {
-        // =========================================================== MMA issuer
-        if (lane == 0) {
-            const uint32_t idesc = make_idesc_f16(TC_M, N_TILE);
-            const uint32_t a_base = smem_u32(smA), b_base = smem_u32(smB);
-            int as = 0, bs = 0, buf = 0;
-            uint32_t aphase = 0, bphase = 0, cphase = 0;
-            bool first = true;
-            for (int tile = blockIdx.x; tile < n_tiles; tile += gridDim.x) {
-                int ph = 0;
-                if (w_resident) bs = 0;
-                for (int g = 0; g < n_groups; ++g) {
-                    mbar_wait(acc_empty + buf, cphase ^ 1);
-                    tc_fence_after_sync();
-                    const uint32_t d_tmem = tmem_base + (uint32_t)(buf * BUF_COLS);
-                    uint32_t accum = 0;
-                    const int u_end = min(n_units, (g + 1) * upg);
-                    for (int unit = g * upg; unit < u_end; ++unit) {
-                        mbar_wait(a_full + as, aphase);
-                        tc_fence_after_sync();
-                        const uint32_t a_hi0 = a_base + as * L.a_stage;
-                        const uint32_t a_lo0 = a_hi0 + L.a_rows * 128;
-                        // K steps of 16 channels: 4 for a full 64-channel stage, 2 when only its first half exists
-                        const int ksteps = (2 * (unit / S) + 1 < n_chunks) ? 4 : 2;
-                        int q = 0;
-                        for (int k = ph; k < K; k += S, ++q) {
-                            if (!w_resident || first) {
-                                mbar_wait(b_full + bs, bphase);
-                                tc_fence_after_sync();
-                            }
-                            const uint32_t b_hi0 = b_base + bs * L.b_stage;
-                            const uint32_t b_lo0 = b_hi0 + N_TILE * 128;
-                            if (!(p.dbg & 32))
-#pragma unroll
-                            for (int ks = 0; ks < 4; ++ks) {
-                                if (ks < ksteps) {
-                                    const uint64_t da_hi = make_desc_k_sw128(a_hi0 + q * 128 + ks * 32);
-                                    const uint64_t da_lo = make_desc_k_sw128(a_lo0 + q * 128 + ks * 32);
-                                    const uint64_t db_hi = make_desc_k_sw128(b_hi0 + ks * 32);
-                                    const uint64_t db_lo = make_desc_k_sw128(b_lo0 + ks * 32);
-                                    mma_f16_ss(d_tmem, da_lo, db_hi, idesc, accum);
-                                    accum = 1;
-                                    mma_f16_ss(d_tmem, da_hi, db_lo, idesc, 1);
-                                    mma_f16_ss(d_tmem, da_hi, db_hi, idesc, 1);
-                                }
-                            }
-                            if (!w_resident) mma_commit(b_empty + bs);
-                            if (++bs == nb_stages) { bs = 0; bphase ^= 1; }
-                        }
-                        mma_commit(a_empty + as);
-                        if (++as == na_stages) { as = 0; aphase ^= 1; }
-                        if (++ph == S) ph = 0;
-                    }
-                    mma_commit(acc_full + buf);
-                    if (++buf == n_acc) { buf = 0; cphase ^= 1; }
-                }
-                first = false;
-            }
-        }
-    } else if (warp == 22) {
         // =========================================================== raw activation tiles via TMA (cp.async.bulk.tensor)
         if (lane == 0 && nraw > 0 && !(p.dbg & 512)) {
             const uint32_t row_bytes = (uint32_t)(L.a_rows * raw_pitch);
@@ -531,173 +456,172 @@ __global__ void __launch_bounds__(TC_THREADS, 1) conv1d_tc_kernel(const __grid_c
                     }
             }
         }
-    } else {
-        // =========================================================== accumulator warps: fold groups, epilogue
-        const int quad = warp & 3;                                   // a warp may only touch TMEM lanes 32*(warp%4)..+31
-        const uint32_t lane_base = (uint32_t)(quad * 32) << 16;
-        const uint32_t tot_base = tmem_base + lane_base + (uint32_t)(n_acc * BUF_COLS);
-        int buf = 0;
-        uint32_t cphase = 0;
+    } else if (warp >= TC_CONS_WARP0) {
+        // =========================================================== consumer warpgroups: wgmma issue, group fold, epilogue
+        constexpr int NA = N_TILE / 2;                            // accumulator registers per thread (m64 x N_TILE per warpgroup)
+        const int cw = warp - TC_CONS_WARP0;                      // 0..7
+        const int wg = cw >> 2;                                   // tile rows 64*wg .. 64*wg + 63
+        const int ctid = tid - TC_CONS_WARP0 * 32;                // 0..255
+        const bool leader = (tid & 127) == 0;                     // one arrival per warpgroup on the ring barriers
+        const uint32_t a_base = smem_u32(smA) + (uint32_t)(wg * 64 * 128), b_base = smem_u32(smB);
+        const int r_lo = wg * 64 + (cw & 3) * 16 + (lane >> 2);   // accumulator rows of this thread: r_lo, r_lo + 8
+        const int cq = 2 * (lane & 3);                            // first of its two columns in every 8-column group
         // 2-D plain convs (no phase scatter, no padded columns) store [pseudo-clip][t][C_out] like a 1-D layer
         const bool plain_out = FREQ && p.fq.FR == 1 && p.fq.TR == 1 && p.fq.c_store == p.C_out;
         const float out_scale = p.tc_out_scale;
         // fused GroupNorm finalisation: partials of the current clip written by this CTA since the last report
         int fin_clip = -1, fin_local = 0;
         auto fin_flush = [&]() {
-            // all 128 accumulator threads call this together.  Report this CTA's partial count for fin_clip; whoever completes the
+            // all 256 consumer threads call this together.  Report this CTA's partial count for fin_clip; whoever completes the
             // clip reduces ALL its partials in a fixed order (independent of which CTA does it) and writes stats + affine.
             if (fin_clip < 0 || fin_local == 0) return;
-            int* flag = reinterpret_cast<int*>(red + 8);
-            if (quad == 0 && lane == 0) {
+            int* flag = reinterpret_cast<int*>(red + 16);
+            if (ctid == 0) {
                 __threadfence();                                         // this CTA's partials before the count
                 const int old = atomicAdd(p.fin_counter + fin_clip, fin_local);
                 *flag = (old + fin_local == p.fin_parts) ? 1 : 0;
             }
-            asm volatile("bar.sync 1, 128;" ::: "memory");
+            asm volatile("bar.sync 1, 256;" ::: "memory");
             const bool last_cta = *flag != 0;
             if (last_cta) {
                 __threadfence();                                         // the other CTAs' partials after the count
-                const int t128 = quad * 32 + lane;
                 const double* pp = p.partials + (long long)fin_clip * p.fin_parts * 2;
                 double fs = 0.0, fss = 0.0;
-                for (int i = t128; i < p.fin_parts; i += 128) { fs += __ldcg(pp + 2 * i); fss += __ldcg(pp + 2 * i + 1); }
+                for (int i = ctid; i < p.fin_parts; i += 256) { fs += __ldcg(pp + 2 * i); fss += __ldcg(pp + 2 * i + 1); }
 #pragma unroll
                 for (int o = 16; o > 0; o >>= 1) {
                     fs += __shfl_xor_sync(0xffffffffu, fs, o);
                     fss += __shfl_xor_sync(0xffffffffu, fss, o);
                 }
-                asm volatile("bar.sync 1, 128;" ::: "memory");          // everyone has read the flag
-                if (lane == 0) { red[quad * 2] = fs; red[quad * 2 + 1] = fss; }
-                asm volatile("bar.sync 1, 128;" ::: "memory");
-                const double ts = (red[0] + red[2]) + (red[4] + red[6]), tss = (red[1] + red[3]) + (red[5] + red[7]);
+                asm volatile("bar.sync 1, 256;" ::: "memory");          // everyone has read the flag
+                if (lane == 0) { red[cw * 2] = fs; red[cw * 2 + 1] = fss; }
+                asm volatile("bar.sync 1, 256;" ::: "memory");
+                double ts = 0.0, tss = 0.0;
+#pragma unroll
+                for (int w = 0; w < 8; ++w) { ts += red[2 * w]; tss += red[2 * w + 1]; }
                 const double mean_d = ts / p.fin_count;
                 double var = tss / p.fin_count - mean_d * mean_d;
                 if (var < 0.0) var = 0.0;
                 const float mean = (float)mean_d, rstd = (float)(1.0 / sqrt(var + (double)p.fin_eps));
-                if (t128 == 0) {
+                if (ctid == 0) {
                     p.fin_stats[2 * fin_clip] = mean;
                     p.fin_stats[2 * fin_clip + 1] = rstd;
                     p.fin_counter[fin_clip] = 0;                         // ready for the next launch
                 }
                 if (p.fin_coef)
-                    for (int c = t128; c < p.fin_C; c += 128) {
+                    for (int c = ctid; c < p.fin_C; c += 256) {
                         const float a = rstd * p.fin_gamma[c];
                         p.fin_coef[(long long)fin_clip * 2 * p.fin_C + c] = a;
                         p.fin_coef[(long long)fin_clip * 2 * p.fin_C + p.fin_C + c] = p.fin_beta[c] - a * mean;
                     }
             }
-            asm volatile("bar.sync 1, 128;" ::: "memory");              // `red` / flag free again
+            asm volatile("bar.sync 1, 256;" ::: "memory");              // `red` / flag free again
             fin_local = 0;
         };
+        int as = 0, bs = 0;
+        uint32_t aphase = 0, bphase = 0;
+        bool first = true;
+        float acc[NA], tot[NA];
         for (int tile = blockIdx.x; tile < n_tiles; tile += gridDim.x) {
             const TcTile tl = tc_tile(tile, n_nt, n_tt);
-            const int t = tl.tt * TC_M + quad * 32 + lane;
-            const bool row_ok = t < p.T_out;
-            float* orow = p.out + (long long)tl.b * p.out_clip_stride + (long long)t * p.C_out + (long long)tl.nt * N_TILE;
-            const float* bias = p.bias + tl.nt * N_TILE;
-            long long frow = 0;                                       // FREQ: element row of (clip, f_out*FR, t*TR)
+            int ph = 0;
+            if (w_resident) bs = 0;
+            // a ring stage is released once the wgmma that read it have completed: one commit group per tap, at most one
+            // group in flight behind the one just issued
+            int pend_a = -1, pend_b = -1;
+            for (int g = 0; g < n_groups; ++g) {
+                uint32_t accum = 0;
+                const int u_end = min(n_units, (g + 1) * upg);
+                for (int unit = g * upg; unit < u_end; ++unit) {
+                    mbar_wait(a_full + as, aphase);
+                    const uint32_t a_hi0 = a_base + as * L.a_stage;
+                    const uint32_t a_lo0 = a_hi0 + L.a_rows * 128;
+                    // K steps of 16 channels: 4 for a full 64-channel stage, 2 when only its first half exists
+                    const int ksteps = (2 * (unit / S) + 1 < n_chunks) ? 4 : 2;
+                    int q = 0;
+                    for (int k = ph; k < K; k += S, ++q) {
+                        if (!w_resident || first) mbar_wait(b_full + bs, bphase);
+                        const uint32_t b_hi0 = b_base + bs * L.b_stage;
+                        const uint32_t b_lo0 = b_hi0 + N_TILE * 128;
+                        wgmma_fence();
+                        if (!(p.dbg & 32))
+#pragma unroll
+                        for (int ks = 0; ks < 4; ++ks) {
+                            if (ks < ksteps) {
+                                const uint64_t da_hi = make_desc_k_sw128(a_hi0 + q * 128 + ks * 32);
+                                const uint64_t da_lo = make_desc_k_sw128(a_lo0 + q * 128 + ks * 32);
+                                const uint64_t db_hi = make_desc_k_sw128(b_hi0 + ks * 32);
+                                const uint64_t db_lo = make_desc_k_sw128(b_lo0 + ks * 32);
+                                WgmmaF16<N_TILE>::mma(acc, da_lo, db_hi, accum);
+                                accum = 1;
+                                WgmmaF16<N_TILE>::mma(acc, da_hi, db_lo, 1);
+                                WgmmaF16<N_TILE>::mma(acc, da_hi, db_hi, 1);
+                            }
+                        }
+                        wgmma_commit();
+                        wgmma_wait<1>();
+                        if (leader) {
+                            if (pend_b >= 0) mbar_arrive(b_empty + pend_b);
+                            if (pend_a >= 0) mbar_arrive(a_empty + pend_a);
+                        }
+                        pend_b = w_resident ? -1 : bs;
+                        pend_a = -1;
+                        if (++bs == nb_stages) { bs = 0; bphase ^= 1; }
+                    }
+                    pend_a = as;
+                    if (++as == na_stages) { as = 0; aphase ^= 1; }
+                    if (++ph == S) ph = 0;
+                }
+                wgmma_wait<0>();
+                reg_fence(acc);
+                if (leader) {
+                    if (pend_b >= 0) mbar_arrive(b_empty + pend_b);
+                    if (pend_a >= 0) mbar_arrive(a_empty + pend_a);
+                }
+                pend_a = -1; pend_b = -1;
+#pragma unroll
+                for (int i = 0; i < NA; ++i) tot[i] = g == 0 ? acc[i] : tot[i] + acc[i];
+            }
+            first = false;
+            // ---- epilogue: bias, raw store, GroupNorm partial statistics
+            long long frow = 0;                                       // FREQ: element row of (clip, f_out*FR, t = 0)
             if (FREQ) {
                 const int fb = tl.b / p.fq.F_out, ff = tl.b - fb * p.fq.F_out;
-                frow = ((long long)fb * p.fq.F_out * p.fq.FR + (long long)ff * p.fq.FR) * ((long long)p.T_out * p.fq.TR) + (long long)t * p.fq.TR;
+                frow = ((long long)fb * p.fq.F_out * p.fq.FR + (long long)ff * p.fq.FR) * ((long long)p.T_out * p.fq.TR);
             }
+            const float* bias = p.bias + tl.nt * N_TILE;
             float s = 0.f, ss = 0.f;
-            for (int g = 0; g < n_groups; ++g) {
-                const bool last = (g == n_groups - 1);
-                if (p.dbg & 64) mbar_wait(acc_full + buf, cphase); else mbar_wait_backoff(acc_full + buf, cphase, 128);
-                tc_fence_after_sync();
-                if (!(p.dbg & 128))
 #pragma unroll
-                for (int c0 = 0; c0 < N_TILE; c0 += 32) {
-                    uint32_t v[32];
-                    tmem_ld_32x32b_x32(tmem_base + lane_base + (uint32_t)(buf * BUF_COLS + c0), v);
-                    if (g > 0) {
-                        uint32_t tv[32];
-                        tmem_ld_32x32b_x32(tot_base + (uint32_t)c0, tv);
-                        tmem_ld_wait();
+            for (int j = 0; j < N_TILE / 8; ++j) {
+                const int c = 8 * j + cq;
+                const float bias0 = __ldg(bias + c), bias1 = __ldg(bias + c + 1);
 #pragma unroll
-                        for (int j = 0; j < 32; ++j) v[j] = __float_as_uint(__uint_as_float(tv[j]) + __uint_as_float(v[j]));
+                for (int h = 0; h < 2; ++h) {
+                    const int t = tl.tt * TC_M + r_lo + 8 * h;
+                    if (t >= p.T_out) continue;
+                    // exact power-of-two rescale + bias in one rounding (== fl(acc / scale + bias))
+                    float2 o;
+                    o.x = fmaf(tot[4 * j + 2 * h], out_scale, bias0);
+                    o.y = fmaf(tot[4 * j + 2 * h + 1], out_scale, bias1);
+                    s += o.x + o.y;
+                    ss = fmaf(o.x, o.x, ss); ss = fmaf(o.y, o.y, ss);
+                    if (p.dbg & 8) continue;
+                    if (!FREQ || plain_out) {
+                        *reinterpret_cast<float2*>(p.out + (long long)tl.b * p.out_clip_stride + (long long)t * p.C_out + tl.nt * N_TILE + c) = o;
                     } else {
-                        tmem_ld_wait();
-                    }
-                    if (!last) {
-                        tmem_st_32x32b_x32(tot_base + (uint32_t)c0, v);
-                    } else if (!FREQ || plain_out) {
-                        // bias + statistics in registers, then through a swizzled staging tile so that every global store
-                        // instruction of the warp writes whole rows (4 rows x 128 B = 4 L1 wavefronts instead of 32)
-                        uint8_t* stg = smem_raw + L.off_stg + quad * 4096;
 #pragma unroll
-                        for (int j = 0; j < 32; j += 4) {
-                            if (c0 + j < N_TILE) {
-                                float4 o;
-                                o.x = fmaf(__uint_as_float(v[j + 0]), out_scale, __ldg(bias + c0 + j + 0));
-                                o.y = fmaf(__uint_as_float(v[j + 1]), out_scale, __ldg(bias + c0 + j + 1));
-                                o.z = fmaf(__uint_as_float(v[j + 2]), out_scale, __ldg(bias + c0 + j + 2));
-                                o.w = fmaf(__uint_as_float(v[j + 3]), out_scale, __ldg(bias + c0 + j + 3));
-                                if (row_ok) {
-                                    s += (o.x + o.y) + (o.z + o.w);
-                                    ss = fmaf(o.x, o.x, ss); ss = fmaf(o.y, o.y, ss); ss = fmaf(o.z, o.z, ss); ss = fmaf(o.w, o.w, ss);
-                                }
-                                *reinterpret_cast<float4*>(stg + lane * 128 + ((((j >> 2) ^ (lane & 7))) << 4)) = o;
-                            }
-                        }
-                        __syncwarp();
-                        if (!(p.dbg & 8)) {
-                            const int cc = lane & 7;
-                            if (c0 + cc * 4 < N_TILE) {
-                                float* obase = p.out + (long long)tl.b * p.out_clip_stride + (long long)tl.nt * N_TILE + c0 + cc * 4;
-                                const int trow0 = tl.tt * TC_M + quad * 32;
-#pragma unroll
-                                for (int i = 0; i < 8; ++i) {
-                                    const int rr = i * 4 + (lane >> 3);
-                                    if (trow0 + rr < p.T_out)
-                                        *reinterpret_cast<float4*>(obase + (long long)(trow0 + rr) * p.C_out) =
-                                            *reinterpret_cast<const float4*>(stg + rr * 128 + ((cc ^ (rr & 7)) << 4));
-                                }
-                            }
-                        }
-                        __syncwarp();
-                    } else if (row_ok) {
-                        int ph = 0, cch = 0;                          // FREQ: phase and channel of output column c0 + j
-                        {
-                            const int co = tl.nt * N_TILE + c0;
-                            ph = co / p.fq.Cc;
-                            cch = co - ph * p.fq.Cc;
-                        }
-#pragma unroll
-                        for (int j = 0; j < 32; j += 4) {
-                            if (c0 + j < N_TILE) {
-                                float4 o;
-                                // exact power-of-two rescale + bias in one rounding (== fl(acc / scale + bias))
-                                o.x = fmaf(__uint_as_float(v[j + 0]), out_scale, __ldg(bias + c0 + j + 0));
-                                o.y = fmaf(__uint_as_float(v[j + 1]), out_scale, __ldg(bias + c0 + j + 1));
-                                o.z = fmaf(__uint_as_float(v[j + 2]), out_scale, __ldg(bias + c0 + j + 2));
-                                o.w = fmaf(__uint_as_float(v[j + 3]), out_scale, __ldg(bias + c0 + j + 3));
-                                s += (o.x + o.y) + (o.z + o.w);
-                                ss = fmaf(o.x, o.x, ss); ss = fmaf(o.y, o.y, ss); ss = fmaf(o.z, o.z, ss); ss = fmaf(o.w, o.w, ss);
-                                if (p.dbg & 8) {
-                                } else {
-                                    // phase (pf, pt) of a transposed conv lands on row f_out*FR + pf, column t*TR + pt
-                                    const int pf = ph / p.fq.TR, pt = ph - pf * p.fq.TR;
-                                    float* dst = p.out + (frow + (long long)pf * p.T_out * p.fq.TR + pt) * p.fq.c_store + cch;
-                                    if ((p.fq.c_store & 3) == 0) {
-                                        if (cch < p.fq.c_store) *reinterpret_cast<float4*>(dst) = o;   // (padded columns: no store)
-                                    } else {                          // padded n-tile: only the real channels exist in HBM
-                                        if (cch + 0 < p.fq.c_store) dst[0] = o.x;
-                                        if (cch + 1 < p.fq.c_store) dst[1] = o.y;
-                                        if (cch + 2 < p.fq.c_store) dst[2] = o.z;
-                                        if (cch + 3 < p.fq.c_store) dst[3] = o.w;
-                                    }
-                                    cch += 4;
-                                    if (cch >= p.fq.Cc) { cch = 0; ++ph; }
-                                }
+                        for (int e = 0; e < 2; ++e) {
+                            // phase (pf, pt) of a transposed conv lands on row f_out*FR + pf, column t*TR + pt; padded columns of
+                            // the n-tile (channel >= c_store) do not exist in HBM
+                            const int co = tl.nt * N_TILE + c + e;
+                            const int phs = co / p.fq.Cc, cch = co - phs * p.fq.Cc;
+                            if (cch < p.fq.c_store) {
+                                const int pf = phs / p.fq.TR, pt = phs - pf * p.fq.TR;
+                                p.out[(frow + (long long)t * p.fq.TR + (long long)pf * p.T_out * p.fq.TR + pt) * p.fq.c_store + cch] = e ? o.y : o.x;
                             }
                         }
                     }
                 }
-                if (!last) tmem_st_wait();
-                tc_fence_before_sync();
-                mbar_arrive(acc_empty + buf);
-                if (++buf == n_acc) { buf = 0; cphase ^= 1; }
             }
             if (p.partials && !(p.dbg & 16)) {
                 double ds = (double)s, dss = (double)ss;
@@ -706,14 +630,17 @@ __global__ void __launch_bounds__(TC_THREADS, 1) conv1d_tc_kernel(const __grid_c
                     ds += __shfl_xor_sync(0xffffffffu, ds, o);
                     dss += __shfl_xor_sync(0xffffffffu, dss, o);
                 }
-                asm volatile("bar.sync 1, 128;" ::: "memory");      // previous tile's reader is done with `red`
-                if (lane == 0) { red[quad * 2] = ds; red[quad * 2 + 1] = dss; }
-                asm volatile("bar.sync 1, 128;" ::: "memory");
-                if (quad == 0 && lane == 0) {
+                asm volatile("bar.sync 1, 256;" ::: "memory");      // previous tile's reader is done with `red`
+                if (lane == 0) { red[cw * 2] = ds; red[cw * 2 + 1] = dss; }
+                asm volatile("bar.sync 1, 256;" ::: "memory");
+                if (ctid == 0) {
                     const int nparts = n_nt * n_tt;
                     double* dst = p.partials + ((long long)tl.b * nparts + tl.nt * n_tt + tl.tt) * 2;
-                    dst[0] = (red[0] + red[2]) + (red[4] + red[6]);
-                    dst[1] = (red[1] + red[3]) + (red[5] + red[7]);
+                    double ts = 0.0, tss = 0.0;
+#pragma unroll
+                    for (int w = 0; w < 8; ++w) { ts += red[2 * w]; tss += red[2 * w + 1]; }
+                    dst[0] = ts;
+                    dst[1] = tss;
                 }
                 if (p.fin_counter) {
                     const int clip = FREQ ? tl.b / p.fq.F_out : tl.b;
@@ -723,12 +650,6 @@ __global__ void __launch_bounds__(TC_THREADS, 1) conv1d_tc_kernel(const __grid_c
             }
         }
         if (p.fin_counter && p.partials && !(p.dbg & 16)) fin_flush();
-    }
-    tc_fence_before_sync();
-    __syncthreads();
-    if (warp == 16) {
-        tc_fence_after_sync();
-        tmem_dealloc(tmem_base, TMEM_COLS);
     }
 #undef na_stages
 #undef nb_stages
@@ -745,7 +666,6 @@ __global__ void __launch_bounds__(TC_THREADS, 1) conv1d_tc_kernel(const __grid_c
 #undef n_nt
 #undef units_per_tile
 #undef tq_rows
-#undef n_acc
 }
 
 // ------------------------------------------------------------------------------------------ host side
@@ -759,8 +679,9 @@ bool conv_tc_supported_2d(int cin, int C_out_eff, int KT, int ST) {
     return cin_ok && C_out_eff % 16 == 0 && KT >= 1 && ST >= 1 && ((KT - 1) / ST) <= 16;
 }
 
+// at most 64 output channels per tile: a consumer thread keeps N_TILE / 2 accumulators plus as many running totals in registers,
+// and 896 threads leave 72 registers per thread
 int conv_tc_n_tile(int C_out_eff) {
-    if (C_out_eff >= 128 && C_out_eff % 128 == 0) return 128;
     if (C_out_eff % 64 == 0) return 64;
     if (C_out_eff % 32 == 0) return 32;
     return 16;
@@ -772,7 +693,7 @@ int conv_tc_num_parts(int T_out, int C_out_eff) {
 
 static int g_num_sms = 0;
 
-static int g_group_mmas = TC_GROUP_MMAS, g_deep_ring = 1, g_dbg = 0, g_nacc_cap = 0, g_na_tma = 2;
+static int g_group_mmas = TC_GROUP_MMAS, g_deep_ring = 1, g_dbg = 0, g_na_tma = 2;
 
 struct TcPlan { int resident, na, nb, nraw; TcSmemLayout L; bool ok; };
 
@@ -873,12 +794,6 @@ static cudaError_t launch_tc_n(const ConvParams& p, cudaStream_t st, const TcPla
     ka.units_per_tile = ka.n_chunks * p.S;
     ka.tq_rows = p.T_in / p.S;
     ka.raw_pitch = ((FREQ ? p.fq.cin : p.C_in) < TC_KC ? (FREQ ? p.fq.cin : p.C_in) : TC_KC) * 4;
-    // accumulator ring depth: layers whose tile is one accumulation group keep up to 8 tiles in flight between MMA issue and
-    // epilogue; layers that fold groups (deep K) ping-pong between up to 3 accumulators next to the running totals
-    constexpr int BUF_COLS = N_TILE < 32 ? 32 : N_TILE;
-    const int acc_fit = 512 / BUF_COLS;
-    ka.n_acc = ka.n_groups == 1 ? (acc_fit < 8 ? acc_fit : 8) : (acc_fit - 1 < 3 ? acc_fit - 1 : 3);
-    if (g_nacc_cap >= 2 && ka.n_acc > g_nacc_cap) ka.n_acc = g_nacc_cap;       // experiments (FCB_TC_NACC)
     kern<<<grid, TC_THREADS, pl.L.total, st>>>(p, ka, tm0, tm1);
     return cudaGetLastError();
 }
@@ -901,7 +816,6 @@ cudaError_t launch_conv_tc(const ConvParams& p_in, int B, cudaStream_t st, int* 
         if (const char* v = getenv("FCB_TC_GROUP_MMAS")) g_group_mmas = atoi(v) > 0 ? atoi(v) : TC_GROUP_MMAS;
         if (const char* v = getenv("FCB_TC_DEEP_RING")) g_deep_ring = atoi(v) != 0;
         if (const char* v = getenv("FCB_TC_DBG")) g_dbg = atoi(v);      // profiling knock-outs (wrong results)
-        if (const char* v = getenv("FCB_TC_NACC")) g_nacc_cap = atoi(v);
         if (const char* v = getenv("FCB_TC_NA_TMA")) { const int f = atoi(v); if (f == 2 || f == 4) g_na_tma = f; }
         // TMA staging of the activation tiles: cuTensorMapEncodeTiled through the runtime's driver entry point (no -lcuda)
         g_tma_state = -1;
@@ -931,9 +845,8 @@ cudaError_t launch_conv_tc(const ConvParams& p_in, int B, cudaStream_t st, int* 
     // (interior tiles exist when the clip has at least 3 tiles, or for 1x1 layers -- no halo -- always)
     bool want_raw = g_tma_state == 1 && (n_tt >= 3 || (p.K == 1 && p.S == 1 && p.pad_l == 0)) && p.T_in / p.S >= 1 &&
                     (freq ? (p.fq.cin % TC_KC == 0 || (p.fq.cin == 16 && p.fq.KF == 1)) : (p.C_in % TC_KC == 0 || p.C_in == 16));
-    // 2-D layers: built and parity-tested (5-D tensor maps), but measured SLOWER than the per-thread gather at config 4 (r2g: conv
-    // stack 37.3 vs 33.6 ms) -- the K_F-fold re-read of every input row makes the unit stream L2-bound either way and the TMA path
-    // adds a hand-off; opt-in (FCB_TC_TMA2D=1)
+    // 2-D layers: built and parity-tested (5-D tensor maps) but opt-in (FCB_TC_TMA2D=1): the K_F-fold re-read of every input row
+    // makes the unit stream L2-bound either way and the TMA path adds a hand-off
     if (freq && !(getenv("FCB_TC_TMA2D") && atoi(getenv("FCB_TC_TMA2D")) != 0)) want_raw = false;
     TcPlan pl{};
     if (want_raw) {
@@ -956,7 +869,6 @@ cudaError_t launch_conv_tc(const ConvParams& p_in, int B, cudaStream_t st, int* 
         case 16: return launch_tc_modes<16>(p, st, pl, n_tiles, freq, tm0, tm1);
         case 32: return launch_tc_modes<32>(p, st, pl, n_tiles, freq, tm0, tm1);
         case 64: return launch_tc_modes<64>(p, st, pl, n_tiles, freq, tm0, tm1);
-        case 128: return launch_tc_modes<128>(p, st, pl, n_tiles, freq, tm0, tm1);
         default: return cudaErrorInvalidConfiguration;
     }
 }

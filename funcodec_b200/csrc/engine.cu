@@ -84,12 +84,10 @@ struct fcb_handle {
     unsigned* lstm_barrier = nullptr;
     int* fin_counter = nullptr;  // per-clip partial counters of the fused GroupNorm finalisation (conv_tc.cu), zero between launches
     int rvq_sliced = 1;          // "rvq_sliced" option / FCB_RVQ_SLICED: the column-sliced fp32 RVQ kernel (rvq_simt.cu) for D > 260 (the
-                                 // SoundStream YAMLs' D = 512; r2o found that such a D never fit the whole-chunk kernel).  Validated on
-                                 // hardware in r2q (profiles/soundstream_fullwidth_r2q.txt: codes exact on 4 x 300 frames x 32 stages);
-                                 // 0 makes fcb_finalize refuse such a D instead
+                                 // SoundStream YAMLs' D = 512, which does not fit the whole-chunk kernel's shared memory); parity-tested
+                                 // at full width (tests/test_gpu_fullshape.py); 0 makes fcb_finalize refuse such a D instead
     int fuse_stats = 0;          // "fuse_stats" option / FCB_FUSE_STATS=1: GroupNorm finalisation inside the conv kernel.  OFF by default:
-                                 // measured slower at config 2 (r2m: conv stack 11.7 vs 10.8 ms -- the last CTA's serial reduction sits in
-                                 // every launch's tail) and neutral at B = 1; parity-tested, kept as an option
+                                 // the last CTA's serial reduction sits in every launch's tail; parity-tested, kept as an option
     unsigned long long* lstm_trace = nullptr;   // PROFILING ONLY (env FCB_LSTM_TRACE): managed buffer, dumped by fcb_destroy
     bool use_tc = true;      // tensor-core conv path (FCB_DISABLE_TC=1 or fcb_set_option disables it)
     int use_tc2d = 7;        // FreqCodec 2-D layers on the tensor-core path, bit mask of Conv2W::tc_class ("use_tc2d" option)
@@ -214,7 +212,7 @@ float f16_bits_to_f32(uint16_t hb) {
 
 // Tensor-core weight image (conv_tc.cu): for every (n-tile, 64-channel chunk, tap) one hi slab and one lo slab of
 // [n_tile rows (output channels) x 64 fp16] in the canonical K-major SWIZZLE_128B layout, so that a single 1-D bulk copy
-// drops it into shared memory ready for tcgen05.mma kind::f16.  The weights are multiplied by *scale_out = 2^e chosen so that
+// drops it into shared memory ready for the fp16 wgmma.  The weights are multiplied by *scale_out = 2^e chosen so that
 // max|w| lands in [2^13, 2^14) (well inside fp16, and the lo terms of all but negligible weights stay normal numbers);
 // hi = fp16(w * scale), lo = fp16(w * scale - hi).  The image is returned as packed 32-bit words (two fp16 each).
 void build_tc_image_f16(const std::vector<float>& wp /*[K][cin][cout_eff]*/, int K, int cin, int cout_eff, int n_tile,
@@ -1295,7 +1293,7 @@ int do_encode(fcb_handle* h, const float* wav, int B, int L, int n_q, int64_t* c
 // =============================================================================================== C ABI
 extern "C" {
 
-const char* fcb_version(void) { return "funcodec_b200 0.1.0 sm_100a"; }
+const char* fcb_version(void) { return "funcodec_b200 0.1.0 sm_90a"; }
 
 int fcb_create(const fcb_config* cfg, fcb_handle** out) {
     if (!cfg || !out) return FCB_E_INVALID;

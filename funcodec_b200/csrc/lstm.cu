@@ -6,7 +6,7 @@
 // as gx[B][T][4H] with unit-major packed columns (n' = 4*j + gate).  The recurrence
 //     gates = gx[:, t] + h_{t-1} W_hh^T ;  c = sig(f) c + sig(i) tanh(g) ;  h = sig(o) tanh(c)
 // is strictly sequential in t, so the kernel is built around latency:
-//   * grid = H / UNITS CTAs (<= 148, one per SM, cooperative launch), CTA j owns hidden units
+//   * grid = H / UNITS CTAs (<= 132, one per SM, cooperative launch), CTA j owns hidden units
 //     [j*UNITS, (j+1)*UNITS) and keeps its W_hh slice [H][4*UNITS] (128 KB at H=1024) in shared memory for
 //     all T steps -- W_hh is read from HBM/L2 exactly once per layer instead of once per step;
 //   * per step every CTA needs the whole h_{t-1} of a clip group: it is exchanged through global memory (L2)
@@ -22,22 +22,22 @@
 
 #include "common.cuh"
 #include "kernels.h"
-#include "tc_sm100.cuh"
+#include "tc_sm90.cuh"
 
 namespace fcb {
 
 constexpr int LSTM_GB_MAX = 8;    // clips per work item (accumulator tile): 8, or 4 for small batches (more items in flight)
 constexpr int LSTM_NBUF_MAX = 8;  // h ring depth: 2 .. 8 slots, as many as shared memory holds (more independent clip groups in flight)
 constexpr int LSTM_THREADS = 480; // 8 compute warps, up to 3 x 2 cell warps (items round-robin), 1 loader warp: 15 warps keep the
-                                  // 128-register budget of the 16-warp allocation bucket (17 warps drop to 96: measured slower)
+                                  // 128-register budget of the 16-warp allocation bucket (17 warps drop to 96)
 constexpr int LSTM_PAIRS_MAX = 3;
 constexpr int LSTM_MAX_GROUPS = 64;
 
 __device__ __forceinline__ float sigmoidf_(float x) { return 1.0f / (1.0f + expf(-x)); }
 // Gates on the hardware ex2 / rcp units (default; FCB_LSTM_FASTCELL=0 selects expf / tanhf): ~3e-7 relative instead of ~1e-7, a
-// much shorter dependent chain in the cell phase that heads every timestep's critical path.  Measured (r2fc): 17.73 -> 17.44 ms
-// per config-2 step with an IDENTICAL parity table (same 3999 / 4000 frames, waveforms 1.2e-6).
+// much shorter dependent chain in the cell phase that heads every timestep's critical path; the parity suite passes with either.
 __device__ __forceinline__ float rcp_approx(float x) { float y; asm("rcp.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x)); return y; }
+__device__ __forceinline__ float2 ffma2(float2 a, float2 b, float2 c) { return make_float2(fmaf(a.x, b.x, c.x), fmaf(a.y, b.y, c.y)); }
 __device__ __forceinline__ float sigmoid_fast(float x) { return rcp_approx(1.0f + tc::exp2f_approx(-1.4426950408889634f * x)); }
 __device__ __forceinline__ float tanh_fast(float x) { return fmaf(-2.0f, rcp_approx(1.0f + tc::exp2f_approx(2.8853900817779268f * x)), 1.0f); }
 
@@ -110,7 +110,7 @@ __global__ void __launch_bounds__(LSTM_THREADS, 1) lstm_seq_kernel(const LstmSeq
     const int n_items = T * ng;
     const unsigned nctas = gridDim.x;
 
-    // W_hh slice in the FFMA2-friendly layout: for every pair of consecutive k and every unit u two 16-byte records
+    // W_hh slice in the float2-paired layout: for every pair of consecutive k and every unit u two 16-byte records
     //   rec(kp, half, u) = { W[k][u][2*half], W[k+1][u][2*half], W[k][u][2*half+1], W[k+1][u][2*half+1] }
     // so that one LDS.128 yields two (w_k, w_{k+1}) register pairs and lanes u = 0..UNITS-1 read consecutive records.
     if (MMA) {
@@ -217,7 +217,7 @@ __global__ void __launch_bounds__(LSTM_THREADS, 1) lstm_seq_kernel(const LstmSeq
                 if (tid == 0) LSTM_TRACE(i, 4);
                 continue;
             }
-            // packed fp32 FMAs (FFMA2): even-k and odd-k partial sums live in the two halves of a register pair
+            // even-k and odd-k partial sums live in the two halves of a float2 (two independent fmaf chains)
             float2 acc2[4][GB];
 #pragma unroll
             for (int gg = 0; gg < 4; ++gg)
@@ -233,14 +233,14 @@ __global__ void __launch_bounds__(LSTM_THREADS, 1) lstm_seq_kernel(const LstmSeq
                 for (int bb = 0; bb < GB; ++bb) {
                     const float4 h4 = *reinterpret_cast<const float4*>(Hc + bb * H + k0);
                     const float2 h01 = make_float2(h4.x, h4.y), h23 = make_float2(h4.z, h4.w);
-                    acc2[0][bb] = __ffma2_rn(h01, make_float2(wa0.x, wa0.y), acc2[0][bb]);
-                    acc2[1][bb] = __ffma2_rn(h01, make_float2(wa0.z, wa0.w), acc2[1][bb]);
-                    acc2[2][bb] = __ffma2_rn(h01, make_float2(wb0.x, wb0.y), acc2[2][bb]);
-                    acc2[3][bb] = __ffma2_rn(h01, make_float2(wb0.z, wb0.w), acc2[3][bb]);
-                    acc2[0][bb] = __ffma2_rn(h23, make_float2(wa1.x, wa1.y), acc2[0][bb]);
-                    acc2[1][bb] = __ffma2_rn(h23, make_float2(wa1.z, wa1.w), acc2[1][bb]);
-                    acc2[2][bb] = __ffma2_rn(h23, make_float2(wb1.x, wb1.y), acc2[2][bb]);
-                    acc2[3][bb] = __ffma2_rn(h23, make_float2(wb1.z, wb1.w), acc2[3][bb]);
+                    acc2[0][bb] = ffma2(h01, make_float2(wa0.x, wa0.y), acc2[0][bb]);
+                    acc2[1][bb] = ffma2(h01, make_float2(wa0.z, wa0.w), acc2[1][bb]);
+                    acc2[2][bb] = ffma2(h01, make_float2(wb0.x, wb0.y), acc2[2][bb]);
+                    acc2[3][bb] = ffma2(h01, make_float2(wb0.z, wb0.w), acc2[3][bb]);
+                    acc2[0][bb] = ffma2(h23, make_float2(wa1.x, wa1.y), acc2[0][bb]);
+                    acc2[1][bb] = ffma2(h23, make_float2(wa1.z, wa1.w), acc2[1][bb]);
+                    acc2[2][bb] = ffma2(h23, make_float2(wb1.x, wb1.y), acc2[2][bb]);
+                    acc2[3][bb] = ffma2(h23, make_float2(wb1.z, wb1.w), acc2[3][bb]);
                 }
             }
             float acc[4][GB];
@@ -418,9 +418,8 @@ static int lstm_pick_nbuf(int H, int B, int units, int gb, bool ring) {
     return nbuf;
 }
 
-// clip-group size: 8 clips per work item.  4-clip groups (4 independent chains for B = 16) were measured twice: on the 2-slot
-// ring of round 1 (no gain) and with one ring slot per group (r2d: 3.67 vs 3.32 ms per SLSTM at config 2) -- the per-item
-// fixed costs (poll, bulk copy, reduction, publish) outweigh the shorter gate GEMM.
+// clip-group size: 8 clips per work item (FCB_LSTM_GB=4 selects 4-clip groups: more independent chains, but every item pays the
+// fixed costs of poll, bulk copy, reduction and publish).
 static int lstm_pick_gb(int B) {
     (void)B;
     int gb = 8;
@@ -439,8 +438,7 @@ template <int UNITS, int GB, bool MMA>
 static cudaError_t launch_seq(const LstmSeqParams& p, cudaStream_t st) {
     int nbuf = lstm_pick_nbuf(p.H, p.B, UNITS, GB, true);
     // cell pairs: 3 when there are at least 3 independent clip groups to keep busy and the extra exchange buffer fits
-    // per-group loader lanes only pay with many groups (r2f / r2g: config 2 (2 groups) 3.7 vs 3.45 ms, config 4 (4 groups) 8.15 vs
-    // 6.5 ms, config 3 (8 groups) 36.8 vs 38.0 ms per SLSTM)
+    // per-group loader lanes only for many clip groups (>= 8)
     const int ngroups = (p.B + GB - 1) / GB;
     int npair = 2, pload = ngroups >= 8 ? 1 : 0;
     // two compute-warp sets when an item's gate GEMM is small (H <= 512) and there are other groups to work on
@@ -473,7 +471,7 @@ cudaError_t launch_lstm_seq(const LstmSeqParams& p, cudaStream_t st) {
     if (p.H % 4 != 0) return cudaErrorInvalidValue;
     const int units = lstm_pick_units(p.H);
     const int gb = lstm_pick_gb(p.B);
-    bool mma = p.whh_scale > 0.f;                     // tensor-core gate GEMM (default); FCB_LSTM_MMA=0: the fp32 FFMA2 path
+    bool mma = p.whh_scale > 0.f;                     // tensor-core gate GEMM (default); FCB_LSTM_MMA=0: the fp32 FMA path
     if (const char* v = getenv("FCB_LSTM_MMA")) mma = mma && atoi(v) != 0;
     if (units == 8 && gb == 8) return mma ? launch_seq<8, 8, true>(p, st) : launch_seq<8, 8, false>(p, st);
     if (units == 8 && gb == 4) return launch_seq<8, 4, false>(p, st);

@@ -1,4 +1,4 @@
-// Residual vector quantizer with the nearest-codeword search on the tensor cores (tcgen05.mma kind::tf32,
+// Residual vector quantizer with the nearest-codeword search on the tensor cores (wgmma m64n128k8 tf32,
 // 3xTF32 split) and EXACT fp32 re-scoring of near-ties, all n_q stages in one kernel.
 //
 // Reference: DistributedResidualVectorQuantization.forward (eval) funcodec/modules/quantization/ddp_core_vq.py:367-418,
@@ -8,9 +8,10 @@
 //   * the residual lives in shared memory as the 3xTF32 operand itself: hi and lo slabs (4 chunks of 32 dims,
 //     canonical SWIZZLE_128B K-major), and hi + lo == the fp32 residual EXACTLY, so no separate copy is kept;
 //   * per stage the [K][D] codebook streams through a shared-memory ring as pre-split, pre-swizzled slab images
-//     (one cp.async.bulk per 128-codeword x 32-dim slab), the MMA warp produces dot[128 rows x 128 codewords]
-//     tiles into two ping-pong TMEM accumulators (48 chained MMAs each), and the 4 epilogue warps (TMEM lane ==
-//     row) evaluate t = (|x|^2 - 2*dot) + |c|^2 in the reference's fp32 order and keep the two best (value, index);
+//     (one cp.async.bulk per 128-codeword x 32-dim slab); the compute warpgroup produces dot[128 rows x 128 codewords]
+//     tiles in registers (two m64 halves, 48 chained MMAs per accumulator for D = 128), evaluates
+//     t = (|x|^2 - 2*dot) + |c|^2 in the reference's fp32 order and keeps the two best (value, index) of every row it holds,
+//     merged across the 4 threads that share a row ((value, index) order == the reference's first minimal index);
 //   * the tensor-core dot carries ~1e-5 absolute error, so whenever best and runner-up are closer than
 //     RESCORE_TOL both are re-scored with the exact sequential-fp32 dot product of the SIMT kernel (rvq_simt.cu) and
 //     compared with the first-index tie-break: decisions equal the fp32 path's unless three candidates fall inside
@@ -18,9 +19,10 @@
 //   * dequantize + residual update (ddp_core_vq.py:407-408) re-split the residual in place; the quantized sum is
 //     rebuilt afterwards from the codes by embed_sum_kernel in the reference's accumulation order.
 // FLOPs per launch: 2 * rows * K * D * n_q (x3 tensor passes); bytes: rows*D*4 in, codes out -> tensor-bound.
+#include <climits>
 #include "common.cuh"
 #include "kernels.h"
-#include "tc_sm100.cuh"
+#include "tc_sm90.cuh"
 
 namespace fcb {
 
@@ -29,12 +31,12 @@ using namespace tc;
 constexpr int RQ_M = 128;           // rows per CTA
 constexpr int RQ_N = RVQ_TC_N;      // codewords per MMA tile (measured: 64-wide tiles with a 4-deep ring are 35% slower)
 constexpr int RQ_NB = 2;            // codebook slab ring depth
-constexpr int RQ_THREADS = 192;     // 4 epilogue warps, copy warp, MMA warp
+constexpr int RQ_THREADS = 160;     // compute warpgroup (wgmma issue, scoring, residual update), copy warp
 constexpr float RQ_RESCORE_TOL = 4e-3f;
 
 struct RqSmem {
     int a_slab;        // bytes of one (hi or lo) chunk slab: 128 rows x 128 B
-    int off_b, off_cc, off_xx, off_idx, off_bar, total;
+    int off_b, off_cc, off_xx, off_idx, off_cand, off_bar, total;
 };
 
 __host__ __device__ inline RqSmem rq_layout(int D, int K) {
@@ -45,8 +47,9 @@ __host__ __device__ inline RqSmem rq_layout(int D, int K) {
     L.off_cc = L.off_b + RQ_NB * 2 * RQ_N * 128;      // B ring: [stage][hi|lo][128 x 128 B]
     L.off_xx = L.off_cc + K * 4;
     L.off_idx = L.off_xx + RQ_M * 4;
-    L.off_bar = (L.off_idx + RQ_M * 4 + 15) & ~15;
-    L.total = L.off_bar + 8 * (2 * RQ_NB + 4 + 1) + 16;
+    L.off_cand = L.off_idx + RQ_M * 4;                // per-row best / runner-up: values [2][128], indices [2][128]
+    L.off_bar = (L.off_cand + 4 * RQ_M * 4 + 15) & ~15;
+    L.total = L.off_bar + 8 * (2 * RQ_NB) + 16;
     return L;
 }
 
@@ -65,25 +68,19 @@ __global__ void __launch_bounds__(RQ_THREADS, 1) rvq_tc_kernel(const RvqParams p
     float* cc_s = reinterpret_cast<float*>(smem_raw + L.off_cc);
     float* xx_s = reinterpret_cast<float*>(smem_raw + L.off_xx);
     int* idx_s = reinterpret_cast<int*>(smem_raw + L.off_idx);
+    float* cv1_s = reinterpret_cast<float*>(smem_raw + L.off_cand);
+    float* cv2_s = cv1_s + RQ_M;
+    int* ci1_s = reinterpret_cast<int*>(cv2_s + RQ_M);
+    int* ci2_s = ci1_s + RQ_M;
     uint64_t* bars = reinterpret_cast<uint64_t*>(smem_raw + L.off_bar);
     uint64_t* b_full = bars;                    // [RQ_NB]
     uint64_t* b_empty = b_full + RQ_NB;         // [RQ_NB]
-    uint64_t* acc_full = b_empty + RQ_NB;       // [2]
-    uint64_t* acc_empty = acc_full + 2;         // [2]
-    uint64_t* a_ready = acc_empty + 2;          // [1] residual slabs (re)written for the stage
-    uint32_t* tmem_ptr = reinterpret_cast<uint32_t*>(a_ready + 1);
 
     if (tid == 0) {
         for (int i = 0; i < RQ_NB; ++i) { mbar_init(b_full + i, 1); mbar_init(b_empty + i, 1); }
-        for (int i = 0; i < 2; ++i) { mbar_init(acc_full + i, 1); mbar_init(acc_empty + i, 128); }
-        mbar_init(a_ready, 128);
         mbar_fence_init();
     }
-    if (warp == 4) tmem_alloc(tmem_ptr, 2 * RQ_N);
-    tc_fence_before_sync();
     __syncthreads();
-    tc_fence_after_sync();
-    const uint32_t tmem_base = *tmem_ptr;
     const long long slab_bytes = 2LL * RQ_N * 128;      // one (n-tile, chunk) hi+lo image
 
     if (warp < 4) {
@@ -118,10 +115,10 @@ __global__ void __launch_bounds__(RQ_THREADS, 1) rvq_tc_kernel(const RvqParams p
                 *reinterpret_cast<float4*>(lo + o) = l;
             }
         }
-        const int quad = warp & 3;
-        const uint32_t lane_base = (uint32_t)(quad * 32) << 16;
-        const int myrow = quad * 32 + lane;                 // TMEM lane == row of this thread
-        long long tcount = 0;                                 // global dist-tile counter (stage-major)
+        const int myrow = tid;                              // row of this thread for the re-scoring and the code store
+        const uint32_t a_base = smem_u32(smA), b_base = smem_u32(smB);
+        long long it = 0;                                   // codebook slab counter (the copy warp's order)
+        auto lex_lt = [](float va, int ia, float vb, int ib) { return va < vb || (va == vb && ia < ib); };
         for (int q = 0; q < p.n_q; ++q) {
             const float* E = p.embed + (long long)q * K * D;
             // ---- |x|^2 in the SIMT kernel's order (8 lanes per row, stride-8 dims, xor-shuffle 1,2,4) and |c|^2
@@ -140,33 +137,94 @@ __global__ void __launch_bounds__(RQ_THREADS, 1) rvq_tc_kernel(const RvqParams p
                 if (jchunk == 0) xx_s[r] = s;
             }
             for (int c = tid; c < K; c += 128) cc_s[c] = __ldg(p.cnorm + (long long)q * K + c);
-            fence_proxy_async_smem();
-            mbar_arrive(a_ready);                             // slabs of this stage are final -> MMA may start
+            fence_proxy_async_smem();                         // slabs of this stage are final -> visible to the wgmma
             asm volatile("bar.sync 1, 128;" ::: "memory");
             const float xx = xx_s[myrow];
-            float v1 = 3.402823466e38f, v2 = 3.402823466e38f;
-            int i1 = 0, i2 = -1;       // a NaN row replaces nothing: index 0, like the reference's max() over NaNs; no OOB gather
-            for (int nt = 0; nt < n_nt; ++nt, ++tcount) {
-                const int buf = (int)(tcount & 1);
-                mbar_wait_backoff(acc_full + buf, (uint32_t)((tcount >> 1) & 1), 64);
-                tc_fence_after_sync();
+            // accumulator rows of this thread: 64*h + 16*warp + lane/4 + 8*e (h: 64-row half, e: fragment row), k = 2*h + e;
+            // best / runner-up per row as (value, index), index INT_MAX = none yet
+            float xr[4], bv1[4], bv2[4];
+            int bi1[4], bi2[4];
 #pragma unroll
-                for (int c0 = 0; c0 < RQ_N; c0 += 32) {
-                    uint32_t v[32];
-                    tmem_ld_32x32b_x32(tmem_base + lane_base + (uint32_t)(buf * RQ_N + c0), v);
-                    tmem_ld_wait();
+            for (int k = 0; k < 4; ++k) {
+                xr[k] = xx_s[64 * (k >> 1) + 16 * warp + (lane >> 2) + 8 * (k & 1)];
+                bv1[k] = 3.402823466e38f; bv2[k] = 3.402823466e38f;
+                bi1[k] = INT_MAX; bi2[k] = INT_MAX;
+            }
+            for (int nt = 0; nt < n_nt; ++nt) {
+                float acc0[RQ_N / 2], acc1[RQ_N / 2];
+                int prev = -1;
+                for (int ch = 0; ch < n_chunks; ++ch, ++it) {
+                    const int bs = (int)(it % RQ_NB);
+                    mbar_wait(b_full + bs, (uint32_t)((it / RQ_NB) & 1));
+                    const uint32_t a_hi0 = a_base + (2 * ch) * L.a_slab, a_lo0 = a_hi0 + L.a_slab;
+                    const uint32_t b_hi0 = b_base + bs * (uint32_t)slab_bytes, b_lo0 = b_hi0 + RQ_N * 128;
+                    wgmma_fence();
 #pragma unroll
-                    for (int j = 0; j < 32; ++j) {
-                        const int c = nt * RQ_N + c0 + j;
-                        const float tv = __fadd_rn(__fsub_rn(xx, 2.0f * __uint_as_float(v[j])), cc_s[c]);
-                        if (tv < v1) { v2 = v1; i2 = i1; v1 = tv; i1 = c; }
-                        else if (tv < v2) { v2 = tv; i2 = c; }
+                    for (int ks = 0; ks < 4; ++ks) {
+                        const uint64_t db_hi = make_desc_k_sw128(b_hi0 + ks * 32), db_lo = make_desc_k_sw128(b_lo0 + ks * 32);
+                        const uint32_t accum = (ch | ks) != 0;
+                        // rows 0-63, then rows 64-127 (64 rows x 128 B further into the slab)
+                        wgmma_m64n128k8_tf32(acc0, make_desc_k_sw128(a_lo0 + ks * 32), db_hi, accum);
+                        wgmma_m64n128k8_tf32(acc0, make_desc_k_sw128(a_hi0 + ks * 32), db_lo, 1);
+                        wgmma_m64n128k8_tf32(acc0, make_desc_k_sw128(a_hi0 + ks * 32), db_hi, 1);
+                        wgmma_m64n128k8_tf32(acc1, make_desc_k_sw128(a_lo0 + 8192 + ks * 32), db_hi, accum);
+                        wgmma_m64n128k8_tf32(acc1, make_desc_k_sw128(a_hi0 + 8192 + ks * 32), db_lo, 1);
+                        wgmma_m64n128k8_tf32(acc1, make_desc_k_sw128(a_hi0 + 8192 + ks * 32), db_hi, 1);
+                    }
+                    wgmma_commit();
+                    wgmma_wait<1>();                           // the previous slab has been read
+                    if (prev >= 0 && tid == 0) mbar_arrive(b_empty + prev);
+                    prev = bs;
+                }
+                wgmma_wait<0>();
+                reg_fence(acc0);
+                reg_fence(acc1);
+                if (tid == 0) mbar_arrive(b_empty + prev);
+                // every thread sees the columns of its rows in ascending order: strict '<' keeps the first minimal index
+                auto scan = [&](const float (&a)[RQ_N / 2], int h) {
+#pragma unroll
+                    for (int j = 0; j < RQ_N / 8; ++j)
+#pragma unroll
+                        for (int e = 0; e < 2; ++e) {
+                            const int k = 2 * h + e;
+#pragma unroll
+                            for (int x = 0; x < 2; ++x) {
+                                const int c = nt * RQ_N + 8 * j + 2 * (lane & 3) + x;
+                                const float tv = __fadd_rn(__fsub_rn(xr[k], 2.0f * a[4 * j + 2 * e + x]), cc_s[c]);
+                                if (tv < bv1[k]) { bv2[k] = bv1[k]; bi2[k] = bi1[k]; bv1[k] = tv; bi1[k] = c; }
+                                else if (tv < bv2[k]) { bv2[k] = tv; bi2[k] = c; }
+                            }
+                        }
+                };
+                scan(acc0, 0);
+                scan(acc1, 1);
+            }
+            // merge the (disjoint, ascending-scanned) candidate pairs of the 4 threads sharing a row in (value, index) order
+#pragma unroll
+            for (int k = 0; k < 4; ++k) {
+#pragma unroll
+                for (int o = 1; o <= 2; o <<= 1) {
+                    const float ov1 = __shfl_xor_sync(0xffffffffu, bv1[k], o), ov2 = __shfl_xor_sync(0xffffffffu, bv2[k], o);
+                    const int oi1 = __shfl_xor_sync(0xffffffffu, bi1[k], o), oi2 = __shfl_xor_sync(0xffffffffu, bi2[k], o);
+                    if (lex_lt(ov1, oi1, bv1[k], bi1[k])) {
+                        if (lex_lt(ov2, oi2, bv1[k], bi1[k])) { bv2[k] = ov2; bi2[k] = oi2; }
+                        else { bv2[k] = bv1[k]; bi2[k] = bi1[k]; }
+                        bv1[k] = ov1; bi1[k] = oi1;
+                    } else if (lex_lt(ov1, oi1, bv2[k], bi2[k])) {
+                        bv2[k] = ov1; bi2[k] = oi1;
                     }
                 }
-                tc_fence_before_sync();
-                mbar_arrive(acc_empty + buf);
+                if ((lane & 3) == 0) {
+                    // a row without any finite score (NaN input) keeps index 0 and no runner-up, like the reference's max()
+                    const int rr = 64 * (k >> 1) + 16 * warp + (lane >> 2) + 8 * (k & 1);
+                    cv1_s[rr] = bv1[k]; ci1_s[rr] = bi1[k] == INT_MAX ? 0 : bi1[k];
+                    cv2_s[rr] = bv2[k]; ci2_s[rr] = bi2[k] == INT_MAX ? -1 : bi2[k];
+                }
             }
+            asm volatile("bar.sync 1, 128;" ::: "memory");
             // ---- exact fp32 re-scoring of near-ties (sequential fmaf chain == rvq_simt.cu)
+            const float v1 = cv1_s[myrow], v2 = cv2_s[myrow];
+            const int i1 = ci1_s[myrow], i2 = ci2_s[myrow];
             int best = i1;
             if (row0 + myrow < M && v2 - v1 < RQ_RESCORE_TOL + 2e-5f * fabsf(v1) && i2 >= 0) {
                 float d1 = 0.f, d2 = 0.f;
@@ -186,7 +244,7 @@ __global__ void __launch_bounds__(RQ_THREADS, 1) rvq_tc_kernel(const RvqParams p
             idx_s[myrow] = best;
             if (row0 + myrow < M) p.codes[(long long)q * M + row0 + myrow] = (long long)best;
             asm volatile("bar.sync 1, 128;" ::: "memory");
-            // ---- dequantize + residual update (all MMAs of the stage have completed: last acc_full was waited on).
+            // ---- dequantize + residual update (all wgmma of the stage have completed).
             // 8 passes of 16 rows; the codeword reads of pass i+1 (L2 latency) are in flight while pass i is re-split.
             {
                 constexpr int MAXCH = 4;                       // D <= 128 on this path
@@ -248,48 +306,6 @@ __global__ void __launch_bounds__(RQ_THREADS, 1) rvq_tc_kernel(const RvqParams p
                     }
             }
         }
-    } else {
-        // =========================================================== MMA issuer
-        if (lane == 0) {
-            const uint32_t idesc = make_idesc_tf32(RQ_M, RQ_N);
-            const uint32_t a_base = smem_u32(smA), b_base = smem_u32(smB);
-            long long it = 0, tcount = 0;
-            for (int q = 0; q < p.n_q; ++q) {
-                mbar_wait(a_ready, (uint32_t)(q & 1));
-                tc_fence_after_sync();
-                for (int nt = 0; nt < n_nt; ++nt, ++tcount) {
-                    const int buf = (int)(tcount & 1);
-                    mbar_wait(acc_empty + buf, (uint32_t)((tcount >> 1) & 1) ^ 1);
-                    tc_fence_after_sync();
-                    const uint32_t d_tmem = tmem_base + (uint32_t)(buf * RQ_N);
-                    uint32_t accum = 0;
-                    for (int ch = 0; ch < n_chunks; ++ch, ++it) {
-                        const int bs = (int)(it % RQ_NB);
-                        mbar_wait(b_full + bs, (uint32_t)((it / RQ_NB) & 1));
-                        tc_fence_after_sync();
-                        const uint32_t a_hi0 = a_base + (2 * ch) * L.a_slab, a_lo0 = a_hi0 + L.a_slab;
-                        const uint32_t b_hi0 = b_base + bs * (uint32_t)slab_bytes, b_lo0 = b_hi0 + RQ_N * 128;
-#pragma unroll
-                        for (int ks = 0; ks < 4; ++ks) {
-                            const uint64_t da_hi = make_desc_k_sw128(a_hi0 + ks * 32), da_lo = make_desc_k_sw128(a_lo0 + ks * 32);
-                            const uint64_t db_hi = make_desc_k_sw128(b_hi0 + ks * 32), db_lo = make_desc_k_sw128(b_lo0 + ks * 32);
-                            mma_tf32_ss(d_tmem, da_lo, db_hi, idesc, accum);
-                            accum = 1;
-                            mma_tf32_ss(d_tmem, da_hi, db_lo, idesc, 1);
-                            mma_tf32_ss(d_tmem, da_hi, db_hi, idesc, 1);
-                        }
-                        mma_commit(b_empty + bs);
-                    }
-                    mma_commit(acc_full + buf);
-                }
-            }
-        }
-    }
-    tc_fence_before_sync();
-    __syncthreads();
-    if (warp == 4) {
-        tc_fence_after_sync();
-        tmem_dealloc(tmem_base, 2 * RQ_N);
     }
 }
 

@@ -1,5 +1,5 @@
 /*
- * funcodec_b200 -- C ABI of the B200-native (sm_100a) codec encode -> RVQ -> decode hot path.
+ * funcodec_b200 -- C ABI of the H100-native (sm_90a) codec encode -> RVQ -> decode hot path.
  *
  * The reference (modelscope/FunCodec) is pure Python and has no FFI; the seam this library sits
  * under is the method seam of its `Encodec` model class (SURVEY.md section 8(b)):
@@ -86,7 +86,7 @@ typedef struct fcb_config {
 
 typedef struct fcb_handle fcb_handle;
 
-/* Library / build identification ("funcodec_b200 x.y sm_100a"). */
+/* Library / build identification ("funcodec_b200 x.y sm_90a"). */
 FCB_API const char* fcb_version(void);
 
 /* Create a model instance bound to the current CUDA device.  Replaces the module construction in
@@ -196,7 +196,7 @@ FCB_API int fcb_set_profiling(fcb_handle* h, int32_t enabled);
 /* Milliseconds spent per phase in the most recent call (synchronises the recorded events). */
 FCB_API int fcb_get_phase_ms(fcb_handle* h, float* ms_out /* [FCB_NUM_PHASES] */);
 
-/* Options (integer valued): "use_tc" 1/0 -- tensor-core (tcgen05) conv path vs fp32 SIMT path; must be set
+/* Options (integer valued): "use_tc" 1/0 -- tensor-core (wgmma) conv path vs fp32 SIMT path; must be set
  * before fcb_finalize to enable, may be cleared at any time.  Env FCB_DISABLE_TC=1 sets the default to 0. */
 /* "use_tc2d" (FreqCodec, arch 1): bit mask of the 2-D layer classes that run on the tensor-core path -- 1: C_in % 32 == 0,
  * 2: C_in < 32 (several frequency taps per 32-channel chunk), 4: C_out padded to 16 (the 32 -> 3 output conv); default 7,
@@ -204,8 +204,7 @@ FCB_API int fcb_get_phase_ms(fcb_handle* h, float* ms_out /* [FCB_NUM_PHASES] */
 /* "stft_tc" 1/0 (default 1; env FCB_STFT_TC): STFT / iSTFT of the FreqCodec front / back end as two tensor-core GEMMs (windowed
  * DFT bases as conv weight images; needs n_fft and hop to be multiples of 32) instead of the direct-DFT kernels.
  * "conv2d_small_cout" 1/0 (default 1; env FCB_CONV2D_SMALL_COUT): halo-tile SIMT kernel for 2-D convs with C_out <= 4 (FreqCodec's
- * 32 -> 3 output conv) instead of the padded tensor-core n-tile.  Both were validated and A/B-timed on a B200 in round 2
- * (profiles/ab_bringup_r2a.txt). */
+ * 32 -> 3 output conv) instead of the padded tensor-core n-tile.  Both are parity-tested against the alternative. */
 FCB_API int fcb_set_option(fcb_handle* h, const char* key, int32_t value);
 
 /* TEST HOOK (tests/test_gpu_layers.py): run ONE packed conv layer, addressed by its reference module prefix

@@ -1,6 +1,6 @@
 """CPU ORACLE for the FreqCodec (mag_phase) variant of the hot path -- BASELINE config 4.  TEST INFRASTRUCTURE ONLY.
 
-Prepared for round 2 (the CUDA path for SURVEY.md §8 rows R19-R20 is not built yet): a functional restatement over
+The checker for the CUDA path of SURVEY.md §8 rows R19-R20: a functional restatement over
 torch CPU ops of `FreqCodec._encode_frame / _decode_frame` (mag_phase branches, funcodec/models/codec_freq.py:330-342,
 365-373,386 and :406-425,446-448), `SEANetEncoder2d` / `SEANetDecoder2d` (funcodec/models/encoder/seanet_encoder.py:252-363,
 funcodec/models/decoder/seanet_decoder.py:244-360) and `SConv2d` / `SConvTranspose2d` / `pad2d` / `unpad2d`

@@ -102,24 +102,73 @@ def test_config_from_reference_like_freqcodec():
         config_from_reference_model(m)
 
 
-REF = "/root/reference"
+REF_MODULES = os.path.join(ROOT, "tests", "golden", "reference_modules.json")
 
 
-@pytest.mark.skipif(not os.path.isdir(REF), reason="the reference checkout only exists in the build container")
-def test_config_from_the_real_reference_modules():
-    """integration.config_from_reference_model + state_dict name coverage on the REAL reference `Encodec` (ds640, ds320; built by
-    tools/ref_harness.py from /root/reference): every field matches the preset, every tensor the engine needs is in the
-    reference's state_dict under the same name and shape, and option variants that keep the shapes are refused."""
-    import sys
+def _reference_models():
+    """The reference `Encodec` objects as recorded from the unmodified reference by tools/gen_golden_reference_modules.py:
+    module tree (class names, option attributes, children) and state_dict key -> shape map per preset."""
+    import json
+    with open(REF_MODULES) as f:
+        return json.load(f)
+
+
+class _RefModule:
+    """Stand-in for one recorded reference module: same class name, recorded attributes, children by name (and by index
+    for Sequential / ModuleList), modules() in registration order like nn.Module."""
+
+    def __init__(self, rec):
+        self._children = {}
+        for k, v in rec["attrs"].items():
+            setattr(self, k, tuple(v) if k == "dilation" else v)
+        for name, child in rec["children"]:
+            self._children[name] = _rebuild(child)
+
+    def __getattr__(self, k):
+        ch = self.__dict__.get("_children", {})
+        if k in ch:
+            return ch[k]
+        raise AttributeError(k)
+
+    def __getitem__(self, i):
+        return self._children[str(i)]
+
+    def modules(self):
+        yield self
+        for c in self._children.values():
+            yield from c.modules()
+
+
+def _rebuild(rec):
+    import torch.nn as nn
+    if rec["type"] == "ELU":                 # isinstance checks in integration._check_module_options
+        return nn.ELU(alpha=rec["attrs"]["alpha"])
+    if rec["type"] == "GroupNorm":
+        return nn.GroupNorm(rec["attrs"]["num_groups"], rec["attrs"]["num_channels"])
+    return type(rec["type"], (_RefModule,), {})(rec)
+
+
+def _reference_encodec(rec):
     import torch
-    sys.path.insert(0, os.path.join(ROOT, "tools"))
-    from ref_harness import build_reference_encodec
+    m = _rebuild(rec["tree"])
+    sd = {k: torch.empty(shp, device="meta") for k, shp in rec["state_dict"].items()}
+    m.state_dict = lambda: sd
+    return m
+
+
+def test_config_from_the_real_reference_modules():
+    """integration.config_from_reference_model + state_dict name coverage on the REAL reference `Encodec` (ds320, tiny_ds40,
+    the SoundStream / weight_norm variants; recorded from the unmodified reference in tests/golden/reference_modules.json):
+    every field matches the preset, every tensor the engine needs is in the reference's state_dict under the same name and
+    shape, and option variants that keep the shapes are refused."""
     from funcodec_b200.integration import config_from_reference_model, stacked_codebooks, UnsupportedReferenceModel
     from funcodec_b200.weights import state_dict_shapes
-    for name in ("encodec_16k_n32_ds320", "tiny_ds40", "soundstream_noncausal_small", "soundstream_causal_small",
-                 "weightnorm_lstm_small"):
+    models = _reference_models()["models"]
+    names = ("encodec_16k_n32_ds320", "tiny_ds40", "soundstream_noncausal_small", "soundstream_causal_small", "weightnorm_lstm_small")
+    assert set(names) <= set(models)
+    for name in names:
         cfg = get_config(name)
-        m = build_reference_encodec(cfg)
+        m = _reference_encodec(models[name])
         got = config_from_reference_model(m)
         for f in ("arch", "ratios", "n_filters", "dimension", "kernel_size", "last_kernel_size", "residual_kernel_size",
                   "lstm_layers", "codebook_size", "num_quantizers", "sample_rate", "audio_normalize", "n_residual_layers",
@@ -130,7 +179,7 @@ def test_config_from_the_real_reference_modules():
             assert k in sd and tuple(sd[k].shape) == tuple(shp), (name, k)
         assert tuple(stacked_codebooks(sd).shape) == (cfg.num_quantizers, cfg.codebook_size, cfg.dimension)
     # options that keep parameter names and shapes but change the maths are refused
-    m = build_reference_encodec(get_config("tiny_ds40"))
+    m = _reference_encodec(models["tiny_ds40"])
     m.encoder.model[0].causal = True                   # one causal conv among non-causal ones / causal under GroupNorm
     with pytest.raises(UnsupportedReferenceModel):
         config_from_reference_model(m)
@@ -144,24 +193,19 @@ def test_config_from_the_real_reference_modules():
         config_from_reference_model(m)
 
 
-@pytest.mark.skipif(not os.path.isdir(REF), reason="the reference checkout only exists in the build container")
 def test_use_ddp_false_reference_quantizer_keys():
-    """`use_ddp: false` (core_vq.py:147-150): the reference's own per-layer key names are what stacked_codebooks / fcb_finalize
-    assemble into the [n_q, K, D] codebook tensor."""
-    import sys
+    """`use_ddp: false` (core_vq.py:147-150): the reference's own per-layer key names (recorded from the unmodified
+    reference's ResidualVectorQuantization in tests/golden/reference_modules.json) are what stacked_codebooks /
+    fcb_finalize assemble into the [n_q, K, D] codebook tensor."""
     import torch
-    sys.path.insert(0, os.path.join(ROOT, "tools"))
-    from ref_harness import import_reference
-    import_reference()
-    from funcodec.modules.quantization.core_vq import ResidualVectorQuantization
     from funcodec_b200.integration import stacked_codebooks
-    # (in this checkout CostumeQuantizer(use_ddp=False) itself raises -- vq.py:73-84 passes q0_ds_ratio, which
-    # core_vq.VectorQuantization does not accept -- so the RVQ class is built directly; it sits at quantizer.rq.model)
-    rvq = ResidualVectorQuantization(num_quantizers=3, dim=16, codebook_size=32, decay=0.99, kmeans_init=True, kmeans_iters=10,
-                                     threshold_ema_dead_code=2, quantize_dropout=True, rand_num_quant=[1, 2, 3])
-    sd = {"quantizer.rq.model." + k: v for k, v in rvq.state_dict().items()}
+    rec = _reference_models()["use_ddp_false_rvq"]
+    n_q, D, K = rec["num_quantizers"], rec["dim"], rec["codebook_size"]
+    # the RVQ class sits at quantizer.rq.model
+    sd = {"quantizer.rq.model." + k: torch.zeros(shp) for k, shp in rec["state_dict"].items()}
     assert "quantizer.rq.model.layers.0._codebook.embed" in sd and "quantizer.rq.model.embed" not in sd
-    for i in range(3):
-        sd[f"quantizer.rq.model.layers.{i}._codebook.embed"] = torch.full((32, 16), float(i))
+    for i in range(n_q):
+        assert tuple(sd[f"quantizer.rq.model.layers.{i}._codebook.embed"].shape) == (K, D)
+        sd[f"quantizer.rq.model.layers.{i}._codebook.embed"] = torch.full((K, D), float(i))
     e = stacked_codebooks(sd)
-    assert tuple(e.shape) == (3, 32, 16) and [float(e[i, 0, 0]) for i in range(3)] == [0.0, 1.0, 2.0]
+    assert tuple(e.shape) == (n_q, K, D) and [float(e[i, 0, 0]) for i in range(n_q)] == [0.0, 1.0, 2.0]

@@ -15,7 +15,8 @@ from funcodec_b200.bin import codec_inference as CLI
 from funcodec_b200.kaldi_io import ArkScpWriter, read_mat, read_scp_mats
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-REF_CONF = "/root/reference/egs/LibriTTS/codec/conf"
+# the conf/*.yaml files the reference ships (egs/LibriTTS/codec/conf), stored verbatim
+REF_CONF = os.path.join(ROOT, "tests", "golden", "reference_conf")
 
 
 def stage_argv(stage, d, job=1, batch_size=4, bit_width=16000, indices_save_type="text", sr=16000):
@@ -106,7 +107,6 @@ def test_config_from_yaml_refuses_unbuilt_conv_options(tmp_path, patch):
         CLI.config_from_yaml(path)
 
 
-@pytest.mark.skipif(not os.path.isdir(REF_CONF), reason="the reference checkout only exists in the build container")
 def test_config_from_the_reference_repo_yamls():
     """The YAMLs the reference ships: the two Encodec ones, the two mag_phase FreqCodec ones, the two non-causal SoundStream ones
     (3 dilated residual blocks per stage, no sequence model) and the causal weight_norm SoundStream one map to presets; the
@@ -117,6 +117,7 @@ def test_config_from_the_reference_repo_yamls():
             "soundstream_16k_n32_600k_step.yaml": "soundstream_16k_n32_ds320",
             "freqcodec_mag_phase_16k_n32_600k_step.yaml": "freqcodec_magphase_16k_n32_ds320",
             "freqcodec_mag_phase_16k_n32_600k_step_ds640.yaml": "freqcodec_magphase_16k_n32_ds640"}
+    assert set(want) < set(os.listdir(REF_CONF))
     for fn in sorted(os.listdir(REF_CONF)):
         path = os.path.join(REF_CONF, fn)
         if fn in want:

@@ -23,8 +23,9 @@ def _small(golden_dir):
     from funcodec_b200.encodec import B200Encodec
     if "small" not in _M:
         z = np.load(os.path.join(golden_dir, "freq_magphase_small.npz"))
-        sd = {k[3:]: torch.from_numpy(z[k]) for k in z.files if k.startswith("sd.")}
-        cfg = get_config("freq_small")
+        cfg = get_config(str(z["cfg_name"]))
+        sd = init_state_dict(cfg, int(z["seed"]))
+        assert abs(float(sum(v.double().abs().sum().item() for v in sd.values())) - float(z["sd_checksum"])) <= 1e-6 * float(z["sd_checksum"])
         _M["small"] = (z, cfg, sd, B200Encodec(cfg, sd, "cuda:0"), OracleFreqCodec(sd, list(zip(cfg.ratios_f, cfg.ratios))))
     return _M["small"]
 

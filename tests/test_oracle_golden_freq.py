@@ -9,8 +9,10 @@ from oracle.freqcodec_oracle import OracleFreqCodec
 
 
 def test_freqcodec_magphase_oracle_vs_reference(golden_dir):
+    from funcodec_b200 import get_config, init_state_dict
     z = np.load(os.path.join(golden_dir, "freq_magphase_small.npz"))
-    sd = {k[3:]: torch.from_numpy(z[k]) for k in z.files if k.startswith("sd.")}
+    sd = init_state_dict(get_config(str(z["cfg_name"])), int(z["seed"]))
+    assert abs(float(sum(v.double().abs().sum().item() for v in sd.values())) - float(z["sd_checksum"])) <= 1e-6 * float(z["sd_checksum"])
     o = OracleFreqCodec(sd, [tuple(r) for r in z["ratios"]])
     wav = torch.from_numpy(z["wav"])
     r = o.inference(wav, want_margin=True)

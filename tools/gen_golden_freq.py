@@ -1,6 +1,6 @@
 """Golden vectors for the FreqCodec (mag_phase) path from the UNMODIFIED reference (build container only).
-Weights: the reference modules' own default init under torch.manual_seed, stored in the fixture for the small config
-(a few hundred KB) so the oracle test needs nothing else."""
+Weights: funcodec_b200.weights.init_state_dict(cfg, seed) loaded into the reference modules; the fixtures store the seed and a
+checksum of the weights, not the weights themselves."""
 import os
 import sys
 
@@ -47,26 +47,29 @@ def build(n_filters, dimension, K, nq, ratios, conv_group_ratio=-1, tr_conv_grou
 
 if __name__ == "__main__":
     torch.set_num_threads(8)
+    from funcodec_b200 import get_config, init_state_dict
     ratios = [[4, 1], [4, 1], [4, 2], [4, 1]]
-    m = build(4, 32, 64, 6, ratios)
+    cfg = get_config("freq_small")
+    sd = init_state_dict(cfg, 0)
+    m = build(cfg.n_filters, cfg.dimension, cfg.codebook_size, cfg.num_quantizers, ratios)
+    missing, unexpected = m.load_state_dict(sd, strict=False)
+    assert not unexpected and all(k.split(".")[-1] in ("cluster_size", "embed_avg", "inited", "window") for k in missing), (missing, unexpected)
+    m.quantizer.rq.model.inited.fill_(1)
     g = torch.Generator().manual_seed(8)
     wav = 0.1 * torch.randn(2, 3200 + 57, generator=g)
     with torch.no_grad():
         r = m.inference(wav, need_recon=True, bit_width=None, use_scale=True)
         emb, scale = m._encode(wav.unsqueeze(1))[0]
-    out = dict(wav=wav.numpy(), ratios=np.array(ratios), codes=r["code_indices"][0].numpy().astype(np.int16),
+    out = dict(cfg_name=cfg.name, seed=0, wav=wav.numpy(), ratios=np.array(ratios), codes=r["code_indices"][0].numpy().astype(np.int16),
                quant=r["code_embeddings"][0][0].numpy(), scale=r["code_embeddings"][0][1].numpy(),
-               recon=r["recon_speech"].numpy(), encoder_out=emb.numpy())
-    for k, v in m.state_dict().items():
-        if k.startswith(("encoder.", "decoder.")) or k == "quantizer.rq.model.embed":
-            out["sd." + k] = v.numpy()
+               recon=r["recon_speech"].numpy(), encoder_out=emb.numpy(),
+               sd_checksum=float(sum(v.double().abs().sum().item() for v in sd.values())))
     path = os.path.join(OUT, "freq_magphase_small.npz")
     np.savez_compressed(path, **out)
     print("wrote", path, os.path.getsize(path) // 1024, "KiB", "codes", out["codes"].shape, "recon", out["recon"].shape)
 
     # BASELINE config 4 architecture (repo YAML: n_filters 32, D 128, K 1024, n_q 32, groups = 1) on a short clip; weights
     # are funcodec_b200.weights.init_state_dict(cfg, 0) loaded into the reference module (not stored in the fixture)
-    from funcodec_b200 import get_config, init_state_dict
     cfg = get_config("freqcodec_magphase_16k_n32_ds320")
     sd = init_state_dict(cfg, 0)
     m = build(cfg.n_filters, cfg.dimension, cfg.codebook_size, cfg.num_quantizers, ratios)

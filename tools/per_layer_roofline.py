@@ -1,9 +1,9 @@
 """Per-launch roofline table of the conv stack: lines up the conv launches of one step in an ncu launch summary
-(tools/summarize_launches.py output, e.g. profiles/launch_summary_r2z.txt) with the analytic per-launch work
+(tools/summarize_launches.py output) with the analytic per-launch work
 (funcodec_b200.workload.conv_launches) and prints, per launch: shape, layer-boundary MB and GMAC for the batch, the ncu duration,
 achieved GB/s (and % of the measured HBM peak) and fp32-equivalent TFLOP/s.
 
-  python tools/per_layer_roofline.py profiles/launch_summary_r2z.txt [preset] [B] [samples] [hbm_peak_GBps]
+  python tools/per_layer_roofline.py <launch_summary.txt> [preset] [B] [samples] [hbm_peak_GBps]
 
 The ncu durations are cold-cache and serialised (one kernel at a time, caches flushed between replays): they bound each launch
 from above; the step-level number bench.py reports (all launches back to back, L2 warm between consumer and producer) is ~10 %

@@ -1,5 +1,5 @@
 """Condense `ncu --page raw --csv` into one line per kernel launch with the metrics the roofline needs.
-usage: summarize_ncu_raw.py raw.csv [--traffic-json profiles/conv_traffic.json workload source-file-name]
+usage: summarize_ncu_raw.py raw.csv [--traffic-json <out.json> workload source-file-name]
 (the optional arguments also record dram read + write bytes summed over the listed launches for bench.py's roofline.traffic)"""
 import csv
 import sys
@@ -36,7 +36,7 @@ for row in rd[2:]:
     for key, short in KEYS:
         if key in idx:
             out.append(f"{short}={row[idx[key]]}{units[idx[key]] if short in ('dur', 'dram_rd', 'dram_wr') else ''}")
-    for h_, i_ in idx.items():      # anything tensor-pipe related that is non-zero (tcgen05 shows up under several names)
+    for h_, i_ in idx.items():      # anything tensor-pipe related that is non-zero (the tensor pipe shows up under several names)
         if ("tensor" in h_ or "pipe_tc" in h_ or "tmem" in h_) and h_ not in dict(KEYS):
             v_ = row[i_]
             if v_ not in ("0", "0.000000", "", "n/a"):
