@@ -21,10 +21,12 @@
 //     (TMA engine, 1-D) per (chunk, tap) into a ring, completion on an mbarrier.
 //   * PERSISTENT CTAs (one per SM) walk a static list of (clip, n-tile, time-tile) tiles; every role keeps
 //     running across tile boundaries, so the next tile's loads overlap the previous tile's MMAs and epilogue.
-//   * warp roles (28 warps): 0-7 / 8-15 two producer groups taking alternate units (two units of global
-//     loads in flight; the transform is issue-bound, hence 16 warps); 16 weight copies; 17 raw-tile TMA loads;
-//     20-23 / 24-27 two consumer warpgroups, each issuing the wgmma of 64 of the 128 tile rows (its A view starts
-//     64 rows further into the stage) and running the epilogue of its rows.
+//   * warp roles (5 warpgroups, 640 threads; every role fills whole warpgroups and sets its own register budget with
+//     setmaxnreg at entry): warpgroups 0 / 1 are two producer groups taking alternate units (two units of global loads in
+//     flight); warpgroup 2 is control: warp 8 weight copies, warp 9 raw-tile TMA loads, warps 10-11 idle; warpgroups 3 / 4
+//     are the consumers, each issuing the wgmma of 64 of the 128 tile rows (its A view starts 64 rows further into the
+//     stage) and running the epilogue of its rows.  A consumer issues a tap's 12 (or 6) wgmma back to back as one commit
+//     group, from uniform control flow, and touches its accumulators only after the group's final wait.
 //   * the tensor core adds into its fp32 accumulator with truncation, so a long chain loses ~1 ulp per MMA:
 //     chains are cut every ~48 MMAs and each finished group is folded into running totals (registers) with
 //     round-to-nearest CUDA-core adds; the epilogue (bias, channels-last store, GroupNorm partial sums) reads the totals.
@@ -48,11 +50,18 @@ using namespace tc;
 
 constexpr int TC_M = 128;          // time rows per tile
 constexpr int TC_KC = 32;          // channels per producer unit (half of a 128-byte fp16 swizzle row)
-constexpr int TC_THREADS = 896;    // 16 producer warps (2 groups), copy warp, raw-tile TMA warp, 2 idle, 2 consumer warpgroups
-constexpr int TC_CONS_WARP0 = 20;  // first warp of the consumer warpgroups (warpgroup aligned)
+constexpr int TC_THREADS = 640;    // 2 producer warpgroups, 1 control warpgroup, 2 consumer warpgroups
 constexpr int TC_RAW_MAX = 8;      // raw activation ring (TMA-staged units): at most 8 slots
-constexpr int TC_PROD = 256;       // producer threads per group (one unit)
+constexpr int TC_PROD = 128;       // producer threads per group (one warpgroup, one unit)
+constexpr int TC_PROWS = TC_PROD / 8;   // rows per producer pass (8 threads x 4 channels cover a row's 32 channels)
+constexpr int TC_A_ROWS_MAX = 144; // A slab rows: 128 + (K - 1) / S <= 16 (conv_tc_supported), rounded up to 8
 constexpr int TC_GROUP_MMAS = 48;  // target number of wgmma chained in one accumulator before the fp32 fold
+// Per-thread register budgets (setmaxnreg).  The launch gives every thread 96 (640 x 96 = 61 440, the CTA's pool), split as
+// 128 x (2 x TC_CONS_REGS + 2 x TC_PROD_REGS + TC_CTL_REGS) = 61 440.  Each role is spill-free at its budget: a consumer holds
+// N_TILE / 2 accumulators plus as many running totals (64 at N_TILE = 64), a producer keeps three passes of row loads in flight
+// on the edge path, and the raw-tile TMA warp needs more than 32.
+constexpr int TC_LAUNCH_REGS = 96, TC_PROD_REGS = 96, TC_CTL_REGS = 64, TC_CONS_REGS = 112;
+static_assert(128 * (2 * TC_CONS_REGS + 2 * TC_PROD_REGS + TC_CTL_REGS) <= TC_THREADS * TC_LAUNCH_REGS, "register pool");
 
 // ELU with the hardware exponential (ex2.approx): |error| <= ~2e-7 on the (0, 1] range of exp(x), the same order as
 // one fp32 rounding of the reference's exp(x) - 1.  (The SIMT path keeps expf.)
@@ -116,6 +125,21 @@ __device__ __forceinline__ TcTile tc_tile(int id, int n_nt, int n_tt) {
     return t;
 }
 
+// One tap of a stage as one commit group: KSTEPS k-steps of 16 channels, 3 wgmma each (lo*hi, hi*lo, hi*hi -- the k-order of
+// every output column is fixed by this order).  `accum` = 0 starts a fresh accumulation group with the first MMA.
+template <int N_TILE, int KSTEPS>
+__device__ __forceinline__ void tc_issue_tap(float (&acc)[N_TILE / 2], uint32_t a_hi, uint32_t a_lo, uint32_t b_hi, uint32_t b_lo,
+                                             uint32_t accum) {
+    wgmma_fence();
+#pragma unroll
+    for (int ks = 0; ks < KSTEPS; ++ks) {
+        WgmmaF16<N_TILE>::mma(acc, make_desc_k_sw128(a_lo + ks * 32), make_desc_k_sw128(b_hi + ks * 32), ks == 0 ? accum : 1u);
+        WgmmaF16<N_TILE>::mma(acc, make_desc_k_sw128(a_hi + ks * 32), make_desc_k_sw128(b_lo + ks * 32), 1u);
+        WgmmaF16<N_TILE>::mma(acc, make_desc_k_sw128(a_hi + ks * 32), make_desc_k_sw128(b_hi + ks * 32), 1u);
+    }
+    wgmma_commit();
+}
+
 template <int N_TILE, bool FREQ>
 __global__ void __launch_bounds__(TC_THREADS, 1) conv1d_tc_kernel(const __grid_constant__ ConvParams p, const __grid_constant__ TcArgs ka,
                                                                  const __grid_constant__ CUtensorMap tm0,
@@ -143,12 +167,12 @@ __global__ void __launch_bounds__(TC_THREADS, 1) conv1d_tc_kernel(const __grid_c
     uint8_t* smA = smem_raw;
     uint8_t* smB = smem_raw + L.off_b;
     uint64_t* bars = reinterpret_cast<uint64_t*>(smem_raw + L.off_bar);
-    uint64_t* a_full = bars;                       // [na]   producer arrivals (256 per group that fills the stage)
+    uint64_t* a_full = bars;                       // [na]   producer arrivals (128 per group that fills the stage)
     uint64_t* a_empty = a_full + na_stages;        // [na]   one arrival per consumer warpgroup (its wgmma have read the stage)
     uint64_t* b_full = a_empty + na_stages;        // [nb]   expect_tx
     uint64_t* b_empty = b_full + nb_stages;        // [nb]   one arrival per consumer warpgroup
     uint64_t* raw_full = b_empty + nb_stages;      // [TC_RAW_MAX] expect_tx (TMA tile + coefficient slices)
-    uint64_t* raw_empty = raw_full + TC_RAW_MAX;   // [TC_RAW_MAX] 256 arrivals of the consuming producer group
+    uint64_t* raw_empty = raw_full + TC_RAW_MAX;   // [TC_RAW_MAX] 128 arrivals of the consuming producer group
     double* red = reinterpret_cast<double*>(raw_empty + TC_RAW_MAX);   // [8][2] statistics scratch + finalisation flag
     uint8_t* smR = smem_raw + L.off_raw;
     // TMA-staged units (nraw > 0, 1-D layers): an INTERIOR tile needs only rows inside [0, rows covered by the tensor map) -- no
@@ -175,14 +199,17 @@ __global__ void __launch_bounds__(TC_THREADS, 1) conv1d_tc_kernel(const __grid_c
     }
     __syncthreads();
 
-    if (warp < 16) {
+    const int role = warp >> 2;                     // warpgroup: 0, 1 producers; 2 control; 3, 4 consumers
+    if (role < 2) {
         // =========================================================== producers: transformed A slabs
-        const int grp = warp >> 3;
+        setmaxnreg_dec<TC_PROD_REGS>();
+        const int grp = role;
         const int ptid = tid & (TC_PROD - 1);
         const int jchunk = ptid & 7;                // 4 channels (16 bytes of fp32 in HBM, 8 bytes of fp16 in the slab)
         // rows of a warp: {b, b+1, b+4, b+5}: its four 64-byte half rows land on all 32 banks (2 wavefronts per 8-byte store)
         const int wq = (ptid >> 5), lq = (lane >> 3);
-        const int rsub = ((wq >> 1) << 3) + ((wq & 1) << 1) + (lq & 1) + ((lq >> 1) << 2);      // 32 rows per pass
+        const int rsub = ((wq >> 1) << 3) + ((wq & 1) << 1) + (lq & 1) + ((lq >> 1) << 2);      // TC_PROWS = 16 rows per pass
+        constexpr int NR = TC_A_ROWS_MAX / TC_PROWS;                                             // passes per unit
         const int gt_max = (p.T_out - 1) * S - p.pad_l + (K - 1);
         // this group's cursor over the CTA's global stage sequence (tile-major).  split: both groups fill every stage (group g
         // writes the 32-channel half g); otherwise (one 32-channel chunk) the groups take alternate stages and the ring slot
@@ -251,16 +278,16 @@ __global__ void __launch_bounds__(TC_THREADS, 1) conv1d_tc_kernel(const __grid_c
                     if (p.dbg & 64) mbar_wait(a_empty + as, par); else mbar_wait_backoff(a_empty + as, par, 64);
                     const uint8_t* rrow = rb + rsub * raw_pitch + jchunk * 16;
 #pragma unroll
-                    for (int i = 0; i < 5; ++i) {
-                        const int u = rsub + 32 * i;
+                    for (int i = 0; i < NR; ++i) {
+                        const int u = rsub + TC_PROWS * i;
                         if (u < L.a_rows) {
                             float4 v = make_float4(0.f, 0.f, 0.f, 0.f);
                             if (c_ok) {
-                                const float4 xv = *reinterpret_cast<const float4*>(rrow + i * 32 * raw_pitch);
+                                const float4 xv = *reinterpret_cast<const float4*>(rrow + i * TC_PROWS * raw_pitch);
                                 v.x = fmaf(xv.x, a0.x, b0.x); v.y = fmaf(xv.y, a0.y, b0.y);
                                 v.z = fmaf(xv.z, a0.z, b0.z); v.w = fmaf(xv.w, a0.w, b0.w);
                                 if (has1) {
-                                    const float4 yv = *reinterpret_cast<const float4*>(rrow + L.raw_in1 + i * 32 * raw_pitch);
+                                    const float4 yv = *reinterpret_cast<const float4*>(rrow + L.raw_in1 + i * TC_PROWS * raw_pitch);
                                     v.x = v.x + fmaf(yv.x, a1.x, b1.x); v.y = v.y + fmaf(yv.y, a1.y, b1.y);
                                     v.z = v.z + fmaf(yv.z, a1.z, b1.z); v.w = v.w + fmaf(yv.w, a1.w, b1.w);
                                 }
@@ -309,55 +336,62 @@ __global__ void __launch_bounds__(TC_THREADS, 1) conv1d_tc_kernel(const __grid_c
                     a1.x *= in_scale; a1.y *= in_scale; a1.z *= in_scale; a1.w *= in_scale;
                     b1.x *= in_scale; b1.y *= in_scale; b1.z *= in_scale; b1.w *= in_scale;
                 }
-                // all row loads of the unit are issued before the ring slot is waited for
-                constexpr int NR = 5;                      // a_rows <= 160 = 5 passes of 32 rows
-                float4 xa[NR], xb[NR];
-                bool okr[NR];
+                // row loads go out PB passes at a time (what the producer register budget holds); the first batch is issued
+                // before the ring slot is waited for
+                constexpr int PB = 3;
+                static_assert(NR % PB == 0, "whole batches");
 #pragma unroll
-                for (int i = 0; i < NR; ++i) {
-                    const int u = rsub + 32 * i;
-                    const int gt = (t0 + u) * S + ph - p.pad_l;
-                    bool ok = c_ok && u < L.a_rows && gt <= gt_max;
-                    int src = gt;
-                    if (p.pad_zero) ok = ok && gt >= 0 && gt < p.T_in;
-                    else { src = reflect_index(gt, p.T_ext); ok = ok && src < p.T_in && src >= 0; }
-                    okr[i] = ok;
-                    xa[i] = make_float4(0.f, 0.f, 0.f, 0.f);
-                    xb[i] = xa[i];
-                    if (ok && !(p.dbg & 1)) {
-                        const long long off = (long long)src * pitch + c;
-                        xa[i] = __ldg(reinterpret_cast<const float4*>(xu0 + off));
-                        if (has1) xb[i] = __ldg(reinterpret_cast<const float4*>(xu1 + off));
-                    }
-                }
-                if (p.dbg & 64) mbar_wait(a_empty + as, par); else mbar_wait_backoff(a_empty + as, par, 64);
+                for (int i0 = 0; i0 < NR; i0 += PB) {
+                    float4 xa[PB], xb[PB];
+                    bool okr[PB];
 #pragma unroll
-                for (int i = 0; i < NR; ++i) {
-                    const int u = rsub + 32 * i;
-                    if (u < L.a_rows) {
-                        float4 v = make_float4(0.f, 0.f, 0.f, 0.f);
-                        if (p.dbg & 2) v = xa[i];
-                        else if (okr[i]) {
-                            const float4 xv = xa[i];
-                            v.x = fmaf(xv.x, a0.x, b0.x); v.y = fmaf(xv.y, a0.y, b0.y);
-                            v.z = fmaf(xv.z, a0.z, b0.z); v.w = fmaf(xv.w, a0.w, b0.w);
-                            if (has1) {
-                                const float4 yv = xb[i];
-                                v.x = v.x + fmaf(yv.x, a1.x, b1.x); v.y = v.y + fmaf(yv.y, a1.y, b1.y);
-                                v.z = v.z + fmaf(yv.z, a1.z, b1.z); v.w = v.w + fmaf(yv.w, a1.w, b1.w);
-                            }
-                            if (p.elu) {
-                                v.x = elu_scaled(v.x, p.tc_elu_k, in_scale); v.y = elu_scaled(v.y, p.tc_elu_k, in_scale);
-                                v.z = elu_scaled(v.z, p.tc_elu_k, in_scale); v.w = elu_scaled(v.w, p.tc_elu_k, in_scale);
-                            }
+                    for (int j = 0; j < PB; ++j) {
+                        const int u = rsub + TC_PROWS * (i0 + j);
+                        const int gt = (t0 + u) * S + ph - p.pad_l;
+                        bool ok = c_ok && u < L.a_rows && gt <= gt_max;
+                        int src = gt;
+                        if (p.pad_zero) ok = ok && gt >= 0 && gt < p.T_in;
+                        else { src = reflect_index(gt, p.T_ext); ok = ok && src < p.T_in && src >= 0; }
+                        okr[j] = ok;
+                        xa[j] = make_float4(0.f, 0.f, 0.f, 0.f);
+                        xb[j] = xa[j];
+                        if (ok && !(p.dbg & 1)) {
+                            const long long off = (long long)src * pitch + c;
+                            xa[j] = __ldg(reinterpret_cast<const float4*>(xu0 + off));
+                            if (has1) xb[j] = __ldg(reinterpret_cast<const float4*>(xu1 + off));
                         }
-                        if (p.dbg & 4) continue;
-                        uint2 h, l;
-                        split_f16x2(v.x, v.y, h.x, l.x);
-                        split_f16x2(v.z, v.w, h.y, l.y);
-                        const uint32_t o = (uint32_t)u * 128u + ((c16 ^ (uint32_t)(u & 7)) << 4) + sub8;
-                        *reinterpret_cast<uint2*>(hi + o) = h;
-                        *reinterpret_cast<uint2*>(lo + o) = l;
+                    }
+                    if (i0 == 0) {
+                        if (p.dbg & 64) mbar_wait(a_empty + as, par); else mbar_wait_backoff(a_empty + as, par, 64);
+                    }
+#pragma unroll
+                    for (int j = 0; j < PB; ++j) {
+                        const int u = rsub + TC_PROWS * (i0 + j);
+                        if (u < L.a_rows) {
+                            float4 v = make_float4(0.f, 0.f, 0.f, 0.f);
+                            if (p.dbg & 2) v = xa[j];
+                            else if (okr[j]) {
+                                const float4 xv = xa[j];
+                                v.x = fmaf(xv.x, a0.x, b0.x); v.y = fmaf(xv.y, a0.y, b0.y);
+                                v.z = fmaf(xv.z, a0.z, b0.z); v.w = fmaf(xv.w, a0.w, b0.w);
+                                if (has1) {
+                                    const float4 yv = xb[j];
+                                    v.x = v.x + fmaf(yv.x, a1.x, b1.x); v.y = v.y + fmaf(yv.y, a1.y, b1.y);
+                                    v.z = v.z + fmaf(yv.z, a1.z, b1.z); v.w = v.w + fmaf(yv.w, a1.w, b1.w);
+                                }
+                                if (p.elu) {
+                                    v.x = elu_scaled(v.x, p.tc_elu_k, in_scale); v.y = elu_scaled(v.y, p.tc_elu_k, in_scale);
+                                    v.z = elu_scaled(v.z, p.tc_elu_k, in_scale); v.w = elu_scaled(v.w, p.tc_elu_k, in_scale);
+                                }
+                            }
+                            if (p.dbg & 4) continue;
+                            uint2 h, l;
+                            split_f16x2(v.x, v.y, h.x, l.x);
+                            split_f16x2(v.z, v.w, h.y, l.y);
+                            const uint32_t o = (uint32_t)u * 128u + ((c16 ^ (uint32_t)(u & 7)) << 4) + sub8;
+                            *reinterpret_cast<uint2*>(hi + o) = h;
+                            *reinterpret_cast<uint2*>(lo + o) = l;
+                        }
                     }
                 }
                 fence_proxy_async_smem();
@@ -372,9 +406,11 @@ __global__ void __launch_bounds__(TC_THREADS, 1) conv1d_tc_kernel(const __grid_c
                 unit -= n_units; tile += gridDim.x;
             }
         }
-    } else if (warp == 16) {
-        // =========================================================== weight slabs via the bulk-copy engine
-        if (lane == 0) {
+    } else if (role == 2) {
+        // =========================================================== control warpgroup: weight slabs (warp 8), raw tiles (warp 9)
+        setmaxnreg_dec<TC_CTL_REGS>();
+        if (warp == 8 && lane == 0) {
+            // weight slabs via the bulk-copy engine
             const uint32_t bytes = (uint32_t)L.b_stage;
             int bs = 0;
             uint32_t bphase = 0;
@@ -398,10 +434,8 @@ __global__ void __launch_bounds__(TC_THREADS, 1) conv1d_tc_kernel(const __grid_c
                 }
                 first = false;
             }
-        }
-    } else if (warp == 17) {
-        // =========================================================== raw activation tiles via TMA (cp.async.bulk.tensor)
-        if (lane == 0 && nraw > 0 && !(p.dbg & 512)) {
+        } else if (warp == 9 && lane == 0 && nraw > 0 && !(p.dbg & 512)) {
+            // raw activation tiles via TMA (cp.async.bulk.tensor)
             const uint32_t row_bytes = (uint32_t)(L.a_rows * raw_pitch);
             const uint32_t cbytes = (uint32_t)raw_pitch;
             const uint32_t n_cf = (p.in0.coef ? 2u : 0u) + ((has1 && p.in1.coef) ? 2u : 0u);
@@ -456,12 +490,13 @@ __global__ void __launch_bounds__(TC_THREADS, 1) conv1d_tc_kernel(const __grid_c
                     }
             }
         }
-    } else if (warp >= TC_CONS_WARP0) {
+    } else {
         // =========================================================== consumer warpgroups: wgmma issue, group fold, epilogue
+        setmaxnreg_inc<TC_CONS_REGS>();
         constexpr int NA = N_TILE / 2;                            // accumulator registers per thread (m64 x N_TILE per warpgroup)
-        const int cw = warp - TC_CONS_WARP0;                      // 0..7
+        const int cw = warp - 12;                                 // 0..7
         const int wg = cw >> 2;                                   // tile rows 64*wg .. 64*wg + 63
-        const int ctid = tid - TC_CONS_WARP0 * 32;                // 0..255
+        const int ctid = tid - 12 * 32;                           // 0..255
         const bool leader = (tid & 127) == 0;                     // one arrival per warpgroup on the ring barriers
         const uint32_t a_base = smem_u32(smA) + (uint32_t)(wg * 64 * 128), b_base = smem_u32(smB);
         const int r_lo = wg * 64 + (cw & 3) * 16 + (lane >> 2);   // accumulator rows of this thread: r_lo, r_lo + 8
@@ -537,33 +572,19 @@ __global__ void __launch_bounds__(TC_THREADS, 1) conv1d_tc_kernel(const __grid_c
                     const uint32_t a_hi0 = a_base + as * L.a_stage;
                     const uint32_t a_lo0 = a_hi0 + L.a_rows * 128;
                     // K steps of 16 channels: 4 for a full 64-channel stage, 2 when only its first half exists
-                    const int ksteps = (2 * (unit / S) + 1 < n_chunks) ? 4 : 2;
+                    const bool full_stage = 2 * (unit / S) + 1 < n_chunks;
                     int q = 0;
                     for (int k = ph; k < K; k += S, ++q) {
                         if (!w_resident || first) mbar_wait(b_full + bs, bphase);
                         const uint32_t b_hi0 = b_base + bs * L.b_stage;
                         const uint32_t b_lo0 = b_hi0 + N_TILE * 128;
-                        wgmma_fence();
-                        if (!(p.dbg & 32))
-#pragma unroll
-                        for (int ks = 0; ks < 4; ++ks) {
-                            if (ks < ksteps) {
-                                const uint64_t da_hi = make_desc_k_sw128(a_hi0 + q * 128 + ks * 32);
-                                const uint64_t da_lo = make_desc_k_sw128(a_lo0 + q * 128 + ks * 32);
-                                const uint64_t db_hi = make_desc_k_sw128(b_hi0 + ks * 32);
-                                const uint64_t db_lo = make_desc_k_sw128(b_lo0 + ks * 32);
-                                WgmmaF16<N_TILE>::mma(acc, da_lo, db_hi, accum);
-                                accum = 1;
-                                WgmmaF16<N_TILE>::mma(acc, da_hi, db_lo, 1);
-                                WgmmaF16<N_TILE>::mma(acc, da_hi, db_hi, 1);
-                            }
-                        }
-                        wgmma_commit();
+                        if (full_stage) tc_issue_tap<N_TILE, 4>(acc, a_hi0 + q * 128, a_lo0 + q * 128, b_hi0, b_lo0, accum);
+                        else tc_issue_tap<N_TILE, 2>(acc, a_hi0 + q * 128, a_lo0 + q * 128, b_hi0, b_lo0, accum);
+                        accum = 1;
                         wgmma_wait<1>();
-                        if (leader) {
-                            if (pend_b >= 0) mbar_arrive(b_empty + pend_b);
-                            if (pend_a >= 0) mbar_arrive(a_empty + pend_a);
-                        }
+                        // the previous tap's commit group has completed: release what only it read (predicated, no branch)
+                        mbar_arrive_if(b_empty + pend_b, leader && pend_b >= 0);
+                        mbar_arrive_if(a_empty + pend_a, leader && pend_a >= 0);
                         pend_b = w_resident ? -1 : bs;
                         pend_a = -1;
                         if (++bs == nb_stages) { bs = 0; bphase ^= 1; }
@@ -680,7 +701,8 @@ bool conv_tc_supported_2d(int cin, int C_out_eff, int KT, int ST) {
 }
 
 // at most 64 output channels per tile: a consumer thread keeps N_TILE / 2 accumulators plus as many running totals in registers,
-// and 896 threads leave 72 registers per thread
+// and 128 columns (128 registers of both) do not fit the consumer budget next to spill-free producers (DESIGN.md §11).  The
+// weight packer and the launcher both take the tile width from here.
 int conv_tc_n_tile(int C_out_eff) {
     if (C_out_eff % 64 == 0) return 64;
     if (C_out_eff % 32 == 0) return 32;

@@ -25,6 +25,13 @@ __device__ __forceinline__ void mbar_arrive_expect_tx(uint64_t* bar, uint32_t by
     asm volatile("{\n\t.reg .b64 st;\n\tmbarrier.arrive.expect_tx.shared::cta.b64 st, [%0], %1;\n\t}" ::"r"(smem_u32(bar)), "r"(bytes)
                  : "memory");
 }
+// arrival by the threads whose `pred` is set, as a predicated instruction (no branch: usable between wgmma of one warpgroup)
+__device__ __forceinline__ void mbar_arrive_if(uint64_t* bar, bool pred) {
+    asm volatile("{\n\t.reg .pred p;\n\t.reg .b64 st;\n\tsetp.ne.b32 p, %1, 0;\n\t@p mbarrier.arrive.shared::cta.b64 st, [%0];\n\t}" ::"r"(
+                     smem_u32(bar)),
+                 "r"((uint32_t)pred)
+                 : "memory");
+}
 __device__ __forceinline__ bool mbar_try_wait(uint64_t* bar, uint32_t parity) {
     uint32_t ok;
     asm volatile(
@@ -74,6 +81,14 @@ __device__ __forceinline__ void tma_load_5d(void* dst_smem, const void* tmap, in
         "l"(tmap), "r"(smem_u32(bar)), "r"(c0), "r"(c1), "r"(c2), "r"(c3), "r"(c4)
         : "memory");
 }
+
+// ------------------------------------------------------------------------------------------------ register budgets
+// Executed by all 128 threads of a warpgroup: lower / raise its per-thread register count to R (multiple of 8, 24..256).  The
+// raise waits until the CTA's pool (the launch allocation) has the registers that other warpgroups released.
+template <int R>
+__device__ __forceinline__ void setmaxnreg_dec() { asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(R)); }
+template <int R>
+__device__ __forceinline__ void setmaxnreg_inc() { asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(R)); }
 
 // ------------------------------------------------------------------------------------------------ wgmma
 // Every wgmma below is issued by all 128 threads of a warpgroup; accumulator fragment of m64nN (per warp w of the group, lane l):

@@ -1,11 +1,11 @@
-"""Per-launch roofline table of the conv stack: lines up the conv launches of one step in an ncu launch summary
-(tools/summarize_launches.py output) with the analytic per-launch work
-(funcodec_b200.workload.conv_launches) and prints, per launch: shape, layer-boundary MB and GMAC for the batch, the ncu duration,
+"""Per-launch roofline table of the conv stack: lines up the conv launches of one step in a launch list
+(tools/conv_launch_times.py on the GPU, or tools/summarize_launches.py over an ncu capture) with the analytic per-launch work
+(funcodec_b200.workload.conv_launches) and prints, per launch: shape, layer-boundary MB and GMAC for the batch, the duration,
 achieved GB/s (and % of the measured HBM peak) and fp32-equivalent TFLOP/s.
 
   python tools/per_layer_roofline.py <launch_summary.txt> [preset] [B] [samples] [hbm_peak_GBps]
 
-The ncu durations are cold-cache and serialised (one kernel at a time, caches flushed between replays): they bound each launch
+Durations from an ncu list are cold-cache and serialised (one kernel at a time, caches flushed between replays): they bound each launch
 from above; the step-level number bench.py reports (all launches back to back, L2 warm between consumer and producer) is ~10 %
 lower in sum.  Use the table for the SHAPE of the gap -- which launches sit far from the HBM line -- not for absolute claims."""
 import os
@@ -23,7 +23,7 @@ def main():
     preset = sys.argv[2] if len(sys.argv) > 2 else "encodec_16k_n32_ds640"
     B = int(sys.argv[3]) if len(sys.argv) > 3 else 16
     L = int(sys.argv[4]) if len(sys.argv) > 4 else 160000
-    peak = float(sys.argv[5]) if len(sys.argv) > 5 else 6570.0
+    peak = float(sys.argv[5]) if len(sys.argv) > 5 else 3350.0     # H100 SXM data sheet, HBM3
     durs = []
     for line in open(path):
         m = re.match(r"\s*id\s+\d+\s+([\d.]+) us grid\s+\(.*?\)\s+(.*)$", line)
@@ -32,8 +32,7 @@ def main():
     layers = conv_launches(get_config(preset), L)
     if len(durs) != len(layers):
         raise SystemExit(f"{len(durs)} conv launches in {path}, {len(layers)} in the model of {preset}")
-    print(f"# {preset}, B = {B}, {L} samples per clip; durations from {os.path.basename(path)} (ncu, cold cache, serialised); "
-          f"HBM peak {peak:.0f} GB/s (MEASURED_PEAKS.json)")
+    print(f"# {preset}, B = {B}, {L} samples per clip; durations from {os.path.basename(path)}; HBM peak {peak:.0f} GB/s")
     print(f"{'launch':22s} {'cin->cout k/s':>18s} {'T_out':>7s} {'MB':>8s} {'GMAC':>7s} {'us':>7s} {'GB/s':>7s} {'%HBM':>6s} {'TFLOP/s':>8s}  kernel")
     tot_b = tot_m = tot_t = 0.0
     groups = {}
