@@ -13,20 +13,25 @@
 //     D[t (M = 128 time rows), co (N = n_tile)] = sum_{tap k} sum_{ci} X[t*S + k - pad_l][ci] * W[k][ci][co]
 //   * A (activations): one "unit" = (32-channel chunk, stride phase p): the rows {(t0+u)*S + p - pad_l}
 //     are transformed by a producer group and written (hi and lo slabs) into the canonical SWIZZLE_128B
-//     K-major layout; a ring stage holds a 64-channel chunk, i.e. two units side by side (the two producer groups
-//     each fill one half; layers with a single 32-channel chunk fill half a stage and the groups alternate stages);
+//     K-major layout; a ring stage holds a 64-channel chunk, i.e. two units side by side (with two producer groups each
+//     fills one half, a single group fills half 0 then half 1; layers with a single 32-channel chunk fill half a stage
+//     and the groups alternate stages);
 //     every tap k = q*S + p of that phase is then just a ROW-SHIFTED view (start address
 //     + q*128 B; the hardware swizzle works on absolute address bits) of the same slab -- no im2col copy.
 //   * B (weights): pre-split, pre-swizzled slab images in HBM (engine.cu pack_tc), one cp.async.bulk
 //     (TMA engine, 1-D) per (chunk, tap) into a ring, completion on an mbarrier.
 //   * PERSISTENT CTAs (one per SM) walk a static list of (clip, n-tile, time-tile) tiles; every role keeps
 //     running across tile boundaries, so the next tile's loads overlap the previous tile's MMAs and epilogue.
-//   * warp roles (5 warpgroups, 640 threads; every role fills whole warpgroups and sets its own register budget with
-//     setmaxnreg at entry): warpgroups 0 / 1 are two producer groups taking alternate units (two units of global loads in
-//     flight); warpgroup 2 is control: warp 8 weight copies, warp 9 raw-tile TMA loads, warps 10-11 idle; warpgroups 3 / 4
-//     are the consumers, each issuing the wgmma of 64 of the 128 tile rows (its A view starts 64 rows further into the
-//     stage) and running the epilogue of its rows.  A consumer issues a tap's 12 (or 6) wgmma back to back as one commit
-//     group, from uniform control flow, and touches its accumulators only after the group's final wait.
+//   * warp roles (every role fills whole warpgroups and sets its own register budget with setmaxnreg at entry; TcRoles):
+//     first the producer groups -- two at N_TILE <= 64 (5 warpgroups, 640 threads: two units of global loads in flight, for
+//     the HBM-bound shallow layers), one at N_TILE = 128 (4 warpgroups, 512 threads: its registers go to the consumers'
+//     128-column accumulators); then the control warpgroup: warp 0 weight copies, warp 1 raw-tile TMA loads, warps 2-3
+//     idle; then the two consumer warpgroups, each issuing the wgmma of 64 of the 128 tile rows (its A view starts 64 rows
+//     further into the stage) and running the epilogue of its rows.  A consumer issues a tap's 12 (or 6) wgmma back to back
+//     as one commit group, from uniform control flow, and touches its accumulators only after the group's final wait.
+//   * N_TILE = 128 (1-D layers with C_out % 128 == 0) transforms each activation element once per 128 output columns instead
+//     of once per 64; its epilogue still writes one GroupNorm partial per 64 columns, at the index a 64-column tile would
+//     use, so the statistics (and every output bit) do not depend on the tile width.
 //   * the tensor core adds into its fp32 accumulator with truncation, so a long chain loses ~1 ulp per MMA:
 //     chains are cut every ~48 MMAs and each finished group is folded into running totals (registers) with
 //     round-to-nearest CUDA-core adds; the epilogue (bias, channels-last store, GroupNorm partial sums) reads the totals.
@@ -50,18 +55,35 @@ using namespace tc;
 
 constexpr int TC_M = 128;          // time rows per tile
 constexpr int TC_KC = 32;          // channels per producer unit (half of a 128-byte fp16 swizzle row)
-constexpr int TC_THREADS = 640;    // 2 producer warpgroups, 1 control warpgroup, 2 consumer warpgroups
 constexpr int TC_RAW_MAX = 8;      // raw activation ring (TMA-staged units): at most 8 slots
 constexpr int TC_PROD = 128;       // producer threads per group (one warpgroup, one unit)
 constexpr int TC_PROWS = TC_PROD / 8;   // rows per producer pass (8 threads x 4 channels cover a row's 32 channels)
 constexpr int TC_A_ROWS_MAX = 144; // A slab rows: 128 + (K - 1) / S <= 16 (conv_tc_supported), rounded up to 8
 constexpr int TC_GROUP_MMAS = 48;  // target number of wgmma chained in one accumulator before the fp32 fold
-// Per-thread register budgets (setmaxnreg).  The launch gives every thread 96 (640 x 96 = 61 440, the CTA's pool), split as
-// 128 x (2 x TC_CONS_REGS + 2 x TC_PROD_REGS + TC_CTL_REGS) = 61 440.  Each role is spill-free at its budget: a consumer holds
-// N_TILE / 2 accumulators plus as many running totals (64 at N_TILE = 64), a producer keeps three passes of row loads in flight
-// on the edge path, and the raw-tile TMA warp needs more than 32.
-constexpr int TC_LAUNCH_REGS = 96, TC_PROD_REGS = 96, TC_CTL_REGS = 64, TC_CONS_REGS = 112;
-static_assert(128 * (2 * TC_CONS_REGS + 2 * TC_PROD_REGS + TC_CTL_REGS) <= TC_THREADS * TC_LAUNCH_REGS, "register pool");
+// Warp layout and per-thread register budgets (setmaxnreg) of one tile width, all compile-time.  Every role fills whole
+// warpgroups: PROD_GROUPS producer warpgroups, then the control warpgroup, then the two consumer warpgroups.  The launch gives
+// every thread LAUNCH_REGS (the CTA's pool is THREADS x LAUNCH_REGS), which the roles split among themselves:
+//   * N_TILE <= 64: 5 warpgroups (640 threads x 96 = 61 440): producers 2 x 96, control 64, consumers 2 x 112.  A consumer holds
+//     N_TILE / 2 accumulators plus as many running totals (64 at N_TILE = 64); the shallow (C <= 64) layers are latency- and
+//     HBM-bound and need both producer groups' loads in flight.
+//   * N_TILE = 128: 4 warpgroups (512 threads x 128 = 65 536): one producer group at 112 fills both 32-channel halves of every
+//     stage, control 64, consumers 2 x 168 (64 accumulators + 64 running totals).  Each transformed element now feeds 128
+//     columns, so one producer group carries as much transform work per MAC as two did at N_TILE = 64.
+// Each budget is spill-free as compiled (ptxas is not monotonic in them: pick them by compiling); a producer keeps three passes
+// of row loads in flight on the edge path, and the raw-tile TMA warp needs more than 32.
+template <int N_TILE>
+struct TcRoles {
+    static constexpr int PROD_GROUPS = N_TILE > 64 ? 1 : 2;
+    static constexpr int THREADS = 128 * (PROD_GROUPS + 3);
+    static constexpr int LAUNCH_REGS = 65536 / THREADS / 8 * 8;
+    static constexpr int PROD_REGS = N_TILE > 64 ? 112 : 96, CTL_REGS = 64, CONS_REGS = N_TILE > 64 ? 168 : 112;
+    static constexpr int CTL_WG = PROD_GROUPS;            // warpgroup of the control role; the consumers follow it
+    static constexpr int CONS_WG = PROD_GROUPS + 1;
+    // GroupNorm partials per tile: one per 64 columns, so a layer's partial count and fp64 reduction order do not depend on the
+    // tile width
+    static constexpr int PARTS = N_TILE > 64 ? N_TILE / 64 : 1;
+    static_assert(128 * (2 * CONS_REGS + PROD_GROUPS * PROD_REGS + CTL_REGS) <= THREADS * LAUNCH_REGS, "register pool");
+};
 
 // ELU with the hardware exponential (ex2.approx): |error| <= ~2e-7 on the (0, 1] range of exp(x), the same order as
 // one fp32 rounding of the reference's exp(x) - 1.  (The SIMT path keeps expf.)
@@ -95,7 +117,8 @@ __host__ __device__ inline TcSmemLayout tc_layout(int K, int S, int n_tile, int 
     L.raw_slot = (L.raw_cf + 512 + 127) / 128 * 128;
     L.off_raw = L.off_b + nb * L.b_stage;
     L.off_bar = L.off_raw + nraw * L.raw_slot;
-    L.total = L.off_bar + 8 * (2 * na + 2 * nb + 2 * TC_RAW_MAX) + 160;   // + statistics scratch
+    // + statistics scratch: [partials per tile][8 consumer warps][2] doubles + the finalisation flag
+    L.total = L.off_bar + 8 * (2 * na + 2 * nb + 2 * TC_RAW_MAX) + 128 * (n_tile > 64 ? n_tile / 64 : 1) + 32;
     return L;
 }
 
@@ -141,9 +164,10 @@ __device__ __forceinline__ void tc_issue_tap(float (&acc)[N_TILE / 2], uint32_t 
 }
 
 template <int N_TILE, bool FREQ>
-__global__ void __launch_bounds__(TC_THREADS, 1) conv1d_tc_kernel(const __grid_constant__ ConvParams p, const __grid_constant__ TcArgs ka,
+__global__ void __launch_bounds__(TcRoles<N_TILE>::THREADS, 1) conv1d_tc_kernel(const __grid_constant__ ConvParams p, const __grid_constant__ TcArgs ka,
                                                                  const __grid_constant__ CUtensorMap tm0,
                                                                  const __grid_constant__ CUtensorMap tm1) {
+    using R = TcRoles<N_TILE>;
     extern __shared__ __align__(1024) uint8_t smem_raw[];
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
     const int C_in = p.C_in, K = p.K, S = p.S;
@@ -162,18 +186,18 @@ __global__ void __launch_bounds__(TC_THREADS, 1) conv1d_tc_kernel(const __grid_c
 #define n_groups ka.n_groups
 #define n_tt ka.n_tt
 #define n_nt ka.n_nt
-    const bool split = ka.split != 0;                     // both producer groups fill one stage (32 channels each)
+    const bool split = ka.split != 0;                     // a stage holds two 32-channel units (halves)
 
     uint8_t* smA = smem_raw;
     uint8_t* smB = smem_raw + L.off_b;
     uint64_t* bars = reinterpret_cast<uint64_t*>(smem_raw + L.off_bar);
-    uint64_t* a_full = bars;                       // [na]   producer arrivals (128 per group that fills the stage)
+    uint64_t* a_full = bars;                       // [na]   producer arrivals (128 per 32-channel half written)
     uint64_t* a_empty = a_full + na_stages;        // [na]   one arrival per consumer warpgroup (its wgmma have read the stage)
     uint64_t* b_full = a_empty + na_stages;        // [nb]   expect_tx
     uint64_t* b_empty = b_full + nb_stages;        // [nb]   one arrival per consumer warpgroup
     uint64_t* raw_full = b_empty + nb_stages;      // [TC_RAW_MAX] expect_tx (TMA tile + coefficient slices)
     uint64_t* raw_empty = raw_full + TC_RAW_MAX;   // [TC_RAW_MAX] 128 arrivals of the consuming producer group
-    double* red = reinterpret_cast<double*>(raw_empty + TC_RAW_MAX);   // [8][2] statistics scratch + finalisation flag
+    double* red = reinterpret_cast<double*>(raw_empty + TC_RAW_MAX);   // [PARTS][8][2] statistics scratch + finalisation flag
     uint8_t* smR = smem_raw + L.off_raw;
     // TMA-staged units (nraw > 0, 1-D layers): an INTERIOR tile needs only rows inside [0, rows covered by the tensor map) -- no
     // reflection, no zero padding -- so its units arrive as dense [a_rows][32 channel] boxes through the raw ring; the first / last
@@ -199,10 +223,10 @@ __global__ void __launch_bounds__(TC_THREADS, 1) conv1d_tc_kernel(const __grid_c
     }
     __syncthreads();
 
-    const int role = warp >> 2;                     // warpgroup: 0, 1 producers; 2 control; 3, 4 consumers
-    if (role < 2) {
+    const int role = warp >> 2;                     // warpgroup: producers, then control, then the two consumers
+    if (role < R::PROD_GROUPS) {
         // =========================================================== producers: transformed A slabs
-        setmaxnreg_dec<TC_PROD_REGS>();
+        setmaxnreg_dec<R::PROD_REGS>();
         const int grp = role;
         const int ptid = tid & (TC_PROD - 1);
         const int jchunk = ptid & 7;                // 4 channels (16 bytes of fp32 in HBM, 8 bytes of fp16 in the slab)
@@ -211,11 +235,13 @@ __global__ void __launch_bounds__(TC_THREADS, 1) conv1d_tc_kernel(const __grid_c
         const int rsub = ((wq >> 1) << 3) + ((wq & 1) << 1) + (lq & 1) + ((lq >> 1) << 2);      // TC_PROWS = 16 rows per pass
         constexpr int NR = TC_A_ROWS_MAX / TC_PROWS;                                             // passes per unit
         const int gt_max = (p.T_out - 1) * S - p.pad_l + (K - 1);
-        // this group's cursor over the CTA's global stage sequence (tile-major).  split: both groups fill every stage (group g
-        // writes the 32-channel half g); otherwise (one 32-channel chunk) the groups take alternate stages and the ring slot
-        // advances two at a time (na is even), so no division / modulo is needed in the loop
-        const int step = split ? 1 : 2;
-        const int half = split ? grp : 0;
+        // this group's cursor over the CTA's global stage sequence (tile-major).  split: every stage is filled by both groups
+        // (group g writes the 32-channel half g), or by the single group, half 0 then half 1; otherwise (one 32-channel chunk)
+        // the groups take alternate stages and the ring slot advances PROD_GROUPS at a time (na is even), so no division /
+        // modulo is needed in the loop.  Every written half is one group's 128 arrivals on a_full.
+        const int step = split ? 1 : R::PROD_GROUPS;
+        const int half0 = (split && R::PROD_GROUPS == 2) ? grp : 0;
+        int half = half0;
         int tile = blockIdx.x, unit = split ? 0 : grp;
         int as = unit % na_stages;
         uint32_t aphase = 0;
@@ -397,6 +423,8 @@ __global__ void __launch_bounds__(TC_THREADS, 1) conv1d_tc_kernel(const __grid_c
                 fence_proxy_async_smem();
                 }
                 mbar_arrive(a_full + as);
+                if (R::PROD_GROUPS == 1 && split && half == 0) { half = 1; continue; }   // the stage's second half
+                half = half0;
                 as += step;
                 if (as >= na_stages) { as -= na_stages; aphase ^= 1; }
                 unit += step;
@@ -406,10 +434,10 @@ __global__ void __launch_bounds__(TC_THREADS, 1) conv1d_tc_kernel(const __grid_c
                 unit -= n_units; tile += gridDim.x;
             }
         }
-    } else if (role == 2) {
-        // =========================================================== control warpgroup: weight slabs (warp 8), raw tiles (warp 9)
-        setmaxnreg_dec<TC_CTL_REGS>();
-        if (warp == 8 && lane == 0) {
+    } else if (role == R::CTL_WG) {
+        // =========================================================== control warpgroup: weight slabs (its warp 0), raw tiles (warp 1)
+        setmaxnreg_dec<R::CTL_REGS>();
+        if (warp == 4 * R::CTL_WG && lane == 0) {
             // weight slabs via the bulk-copy engine
             const uint32_t bytes = (uint32_t)L.b_stage;
             int bs = 0;
@@ -434,7 +462,7 @@ __global__ void __launch_bounds__(TC_THREADS, 1) conv1d_tc_kernel(const __grid_c
                 }
                 first = false;
             }
-        } else if (warp == 9 && lane == 0 && nraw > 0 && !(p.dbg & 512)) {
+        } else if (warp == 4 * R::CTL_WG + 1 && lane == 0 && nraw > 0 && !(p.dbg & 512)) {
             // raw activation tiles via TMA (cp.async.bulk.tensor)
             const uint32_t row_bytes = (uint32_t)(L.a_rows * raw_pitch);
             const uint32_t cbytes = (uint32_t)raw_pitch;
@@ -492,11 +520,12 @@ __global__ void __launch_bounds__(TC_THREADS, 1) conv1d_tc_kernel(const __grid_c
         }
     } else {
         // =========================================================== consumer warpgroups: wgmma issue, group fold, epilogue
-        setmaxnreg_inc<TC_CONS_REGS>();
+        setmaxnreg_inc<R::CONS_REGS>();
         constexpr int NA = N_TILE / 2;                            // accumulator registers per thread (m64 x N_TILE per warpgroup)
-        const int cw = warp - 12;                                 // 0..7
+        constexpr int PARTS = R::PARTS;
+        const int cw = warp - 4 * R::CONS_WG;                     // 0..7
         const int wg = cw >> 2;                                   // tile rows 64*wg .. 64*wg + 63
-        const int ctid = tid - 12 * 32;                           // 0..255
+        const int ctid = tid - 128 * R::CONS_WG;                  // 0..255
         const bool leader = (tid & 127) == 0;                     // one arrival per warpgroup on the ring barriers
         const uint32_t a_base = smem_u32(smA) + (uint32_t)(wg * 64 * 128), b_base = smem_u32(smB);
         const int r_lo = wg * 64 + (cw & 3) * 16 + (lane >> 2);   // accumulator rows of this thread: r_lo, r_lo + 8
@@ -510,7 +539,7 @@ __global__ void __launch_bounds__(TC_THREADS, 1) conv1d_tc_kernel(const __grid_c
             // all 256 consumer threads call this together.  Report this CTA's partial count for fin_clip; whoever completes the
             // clip reduces ALL its partials in a fixed order (independent of which CTA does it) and writes stats + affine.
             if (fin_clip < 0 || fin_local == 0) return;
-            int* flag = reinterpret_cast<int*>(red + 16);
+            int* flag = reinterpret_cast<int*>(red + 16 * PARTS);
             if (ctid == 0) {
                 __threadfence();                                         // this CTA's partials before the count
                 const int old = atomicAdd(p.fin_counter + fin_clip, fin_local);
@@ -611,10 +640,13 @@ __global__ void __launch_bounds__(TC_THREADS, 1) conv1d_tc_kernel(const __grid_c
                 frow = ((long long)fb * p.fq.F_out * p.fq.FR + (long long)ff * p.fq.FR) * ((long long)p.T_out * p.fq.TR);
             }
             const float* bias = p.bias + tl.nt * N_TILE;
-            float s = 0.f, ss = 0.f;
+            float s[PARTS], ss[PARTS];                                // per 64-column part of the tile
+#pragma unroll
+            for (int hp = 0; hp < PARTS; ++hp) { s[hp] = 0.f; ss[hp] = 0.f; }
 #pragma unroll
             for (int j = 0; j < N_TILE / 8; ++j) {
                 const int c = 8 * j + cq;
+                const int hp = j * PARTS / (N_TILE / 8);
                 const float bias0 = __ldg(bias + c), bias1 = __ldg(bias + c + 1);
 #pragma unroll
                 for (int h = 0; h < 2; ++h) {
@@ -624,8 +656,8 @@ __global__ void __launch_bounds__(TC_THREADS, 1) conv1d_tc_kernel(const __grid_c
                     float2 o;
                     o.x = fmaf(tot[4 * j + 2 * h], out_scale, bias0);
                     o.y = fmaf(tot[4 * j + 2 * h + 1], out_scale, bias1);
-                    s += o.x + o.y;
-                    ss = fmaf(o.x, o.x, ss); ss = fmaf(o.y, o.y, ss);
+                    s[hp] += o.x + o.y;
+                    ss[hp] = fmaf(o.x, o.x, ss[hp]); ss[hp] = fmaf(o.y, o.y, ss[hp]);
                     if (p.dbg & 8) continue;
                     if (!FREQ || plain_out) {
                         *reinterpret_cast<float2*>(p.out + (long long)tl.b * p.out_clip_stride + (long long)t * p.C_out + tl.nt * N_TILE + c) = o;
@@ -645,28 +677,38 @@ __global__ void __launch_bounds__(TC_THREADS, 1) conv1d_tc_kernel(const __grid_c
                 }
             }
             if (p.partials && !(p.dbg & 16)) {
-                double ds = (double)s, dss = (double)ss;
+                // one partial per 64-column part, at the index a 64-column tile of those columns has: the layer's partials and
+                // their reduction order are the same whatever the tile width
+                double ds[PARTS], dss[PARTS];
 #pragma unroll
-                for (int o = 16; o > 0; o >>= 1) {
-                    ds += __shfl_xor_sync(0xffffffffu, ds, o);
-                    dss += __shfl_xor_sync(0xffffffffu, dss, o);
+                for (int hp = 0; hp < PARTS; ++hp) {
+                    ds[hp] = (double)s[hp]; dss[hp] = (double)ss[hp];
+#pragma unroll
+                    for (int o = 16; o > 0; o >>= 1) {
+                        ds[hp] += __shfl_xor_sync(0xffffffffu, ds[hp], o);
+                        dss[hp] += __shfl_xor_sync(0xffffffffu, dss[hp], o);
+                    }
                 }
                 asm volatile("bar.sync 1, 256;" ::: "memory");      // previous tile's reader is done with `red`
-                if (lane == 0) { red[cw * 2] = ds; red[cw * 2 + 1] = dss; }
+                if (lane == 0) {
+#pragma unroll
+                    for (int hp = 0; hp < PARTS; ++hp) { red[(hp * 8 + cw) * 2] = ds[hp]; red[(hp * 8 + cw) * 2 + 1] = dss[hp]; }
+                }
                 asm volatile("bar.sync 1, 256;" ::: "memory");
-                if (ctid == 0) {
-                    const int nparts = n_nt * n_tt;
-                    double* dst = p.partials + ((long long)tl.b * nparts + tl.nt * n_tt + tl.tt) * 2;
+                if (ctid < PARTS) {
+                    const int hp = ctid;
+                    const int nparts = n_nt * PARTS * n_tt;
+                    double* dst = p.partials + ((long long)tl.b * nparts + (tl.nt * PARTS + hp) * n_tt + tl.tt) * 2;
                     double ts = 0.0, tss = 0.0;
 #pragma unroll
-                    for (int w = 0; w < 8; ++w) { ts += red[2 * w]; tss += red[2 * w + 1]; }
+                    for (int w = 0; w < 8; ++w) { ts += red[(hp * 8 + w) * 2]; tss += red[(hp * 8 + w) * 2 + 1]; }
                     dst[0] = ts;
                     dst[1] = tss;
                 }
                 if (p.fin_counter) {
                     const int clip = FREQ ? tl.b / p.fq.F_out : tl.b;
                     if (clip != fin_clip) { fin_flush(); fin_clip = clip; }
-                    ++fin_local;
+                    fin_local += PARTS;
                 }
             }
         }
@@ -700,17 +742,23 @@ bool conv_tc_supported_2d(int cin, int C_out_eff, int KT, int ST) {
     return cin_ok && C_out_eff % 16 == 0 && KT >= 1 && ST >= 1 && ((KT - 1) / ST) <= 16;
 }
 
-// at most 64 output channels per tile: a consumer thread keeps N_TILE / 2 accumulators plus as many running totals in registers,
-// and 128 columns (128 registers of both) do not fit the consumer budget next to spill-free producers (DESIGN.md §11).  The
-// weight packer and the launcher both take the tile width from here.
-int conv_tc_n_tile(int C_out_eff) {
+// output columns per GroupNorm partial (and per tile up to 64)
+static int tc_part_cols(int C_out_eff) {
     if (C_out_eff % 64 == 0) return 64;
     if (C_out_eff % 32 == 0) return 32;
     return 16;
 }
 
+// Output columns per tile.  1-D layers with C_out_eff % 128 == 0 take 128-column tiles (the 4-warpgroup layout of TcRoles), so
+// each activation element is transformed once per 128 columns; the 2-D mode stays at <= 64.  The weight packer and the launcher
+// both take the tile width from here.
+int conv_tc_n_tile(int C_out_eff, bool freq) {
+    if (!freq && C_out_eff % 128 == 0) return 128;
+    return tc_part_cols(C_out_eff);
+}
+
 int conv_tc_num_parts(int T_out, int C_out_eff) {
-    return ((T_out + TC_M - 1) / TC_M) * (C_out_eff / conv_tc_n_tile(C_out_eff));
+    return ((T_out + TC_M - 1) / TC_M) * (C_out_eff / tc_part_cols(C_out_eff));
 }
 
 static int g_num_sms = 0;
@@ -722,6 +770,8 @@ struct TcPlan { int resident, na, nb, nraw; TcSmemLayout L; bool ok; };
 // shared-memory plan: weights resident (small layers: the whole image of the single n-tile) or streamed through a ring as
 // deep as fits; A ring `na_first` stages (4, else 2) -- with a raw TMA ring the A ring only decouples producers from the MMA
 // issue, so 2 stages suffice and the rest of the shared memory buys prefetch depth (nraw units in flight).
+// At N_TILE = 128 a B stage is 32 KB; the last fallback (na = nb = 2) still fits every supported shape: A 2 x 36 KB (144 rows)
+// + B 2 x 32 KB + two raw slots of a two-input unit (2 x 36.5 KB) + barriers and scratch = 209.5 KB of 225.
 static TcPlan tc_plan(const ConvParams& p, int na_first, bool want_raw, int g_deep_ring) {
     const int limit = 225 * 1024;
     const int n_slabs = ((p.C_in + 2 * TC_KC - 1) / (2 * TC_KC)) * p.K;   // (64-channel stage chunk, tap) weight slabs per n-tile
@@ -816,7 +866,7 @@ static cudaError_t launch_tc_n(const ConvParams& p, cudaStream_t st, const TcPla
     ka.units_per_tile = ka.n_chunks * p.S;
     ka.tq_rows = p.T_in / p.S;
     ka.raw_pitch = ((FREQ ? p.fq.cin : p.C_in) < TC_KC ? (FREQ ? p.fq.cin : p.C_in) : TC_KC) * 4;
-    kern<<<grid, TC_THREADS, pl.L.total, st>>>(p, ka, tm0, tm1);
+    kern<<<grid, TcRoles<N_TILE>::THREADS, pl.L.total, st>>>(p, ka, tm0, tm1);
     return cudaGetLastError();
 }
 
@@ -858,7 +908,7 @@ cudaError_t launch_conv_tc(const ConvParams& p_in, int B, cudaStream_t st, int* 
     p.tc_out_scale = 1.0f / (p.tc_in_scale * p.tc_w_scale);     // powers of two: exact
     p.tc_elu_k = 1.4426950408889634f / p.tc_in_scale;
     const int n_tt = (p.T_out + TC_M - 1) / TC_M, n_nt = p.C_out / p.n_tile;
-    *nparts = n_tt * n_nt;
+    *nparts = n_tt * (p.C_out / tc_part_cols(p.C_out));
     const int n_tiles = n_tt * n_nt * B;
     const bool freq = p.fq.KF > 0;          // B counts pseudo-clips (clips x output frequency rows) in the 2-D mode
     // raw TMA ring: 1-D layers with interior tiles (n_tt >= 3), channel counts the box covers, 16-byte aligned views
@@ -891,6 +941,7 @@ cudaError_t launch_conv_tc(const ConvParams& p_in, int B, cudaStream_t st, int* 
         case 16: return launch_tc_modes<16>(p, st, pl, n_tiles, freq, tm0, tm1);
         case 32: return launch_tc_modes<32>(p, st, pl, n_tiles, freq, tm0, tm1);
         case 64: return launch_tc_modes<64>(p, st, pl, n_tiles, freq, tm0, tm1);
+        case 128: return freq ? cudaErrorInvalidConfiguration : launch_tc_n<128, false>(p, st, pl, n_tiles, tm0, tm1);
         default: return cudaErrorInvalidConfiguration;
     }
 }

@@ -281,7 +281,7 @@ void build_tc_image_tf32(const std::vector<float>& wp /*[K][cin][cout_eff]*/, in
 int pack_tc(fcb_handle* h, const std::vector<float>& wp /*[K][cin][cout_eff]*/, int K, int cin, int cout_eff, ConvW* o) {
     o->n_tile = 0;
     if (!h->use_tc || !conv_tc_supported(cin, cout_eff, K, 1, o->d)) return FCB_OK;   // dilated convs run on the SIMT kernel
-    const int n_tile = conv_tc_n_tile(cout_eff);
+    const int n_tile = conv_tc_n_tile(cout_eff, false);
     std::vector<float> img;
     build_tc_image_f16(wp, K, cin, cout_eff, n_tile, &img, &o->tc_scale);
     FCB_TRY(upload(h, img, &o->w_tc));
@@ -746,7 +746,7 @@ int pack_tc2d(fcb_handle* h, const std::vector<float>& wp, const std::vector<flo
     if (!h->use_tc || !conv_tc_supported_2d(o->cin, cout_tc, kt, o->transposed ? 1 : o->st)) return FCB_OK;
     if (cout_tc != cout_eff && o->transposed) return FCB_OK;
     std::vector<float> img;
-    const int n_tile = conv_tc_n_tile(cout_tc);
+    const int n_tile = conv_tc_n_tile(cout_tc, true);
     if (cout_tc == cout_eff) {
         build_tc_image_f16(wp, kt, ck, cout_eff, n_tile, &img, &o->tc_scale);
         o->bias_tc = nullptr;
@@ -1150,7 +1150,7 @@ int pack_stft_bases(fcb_handle* h) {
         ConvW& o = h->stft_w;
         o.cin = 32; o.cout = cout; o.k = K; o.s = hop / 32;
         std::vector<float> img;
-        const int n_tile = conv_tc_n_tile(cout);
+        const int n_tile = conv_tc_n_tile(cout, false);
         build_tc_image_f16(wp, K, 32, cout, n_tile, &img, &o.tc_scale);
         FCB_TRY(upload(h, img, &o.w_tc));
         FCB_TRY(upload(h, bias, &o.bias));
@@ -1172,7 +1172,7 @@ int pack_stft_bases(fcb_handle* h) {
         ConvW& o = h->istft_w;
         o.cin = cin; o.cout = cout; o.k = 1; o.s = 1;
         std::vector<float> img;
-        const int n_tile = conv_tc_n_tile(cout);
+        const int n_tile = conv_tc_n_tile(cout, false);
         build_tc_image_f16(wp, 1, cin, cout, n_tile, &img, &o.tc_scale);
         FCB_TRY(upload(h, img, &o.w_tc));
         FCB_TRY(upload(h, bias, &o.bias));

@@ -25,7 +25,7 @@ cudaError_t launch_sumsq_partials(const float* x, int B, int L, double* partials
 // conv_tc.cu
 bool conv_tc_supported(int C_in, int C_out_eff, int K, int S, int D);
 bool conv_tc_supported_2d(int cin, int C_out_eff, int KT, int ST);
-int conv_tc_n_tile(int C_out_eff);
+int conv_tc_n_tile(int C_out_eff, bool freq);   // freq: the 2-D (FreqCodec) mode
 int conv_tc_num_parts(int T_out, int C_out_eff);
 cudaError_t launch_conv_tc(const ConvParams& p, int B, cudaStream_t st, int* nparts);
 
