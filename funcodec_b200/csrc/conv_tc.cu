@@ -48,6 +48,7 @@
 #include "kernels.h"
 #include "tc_sm90.cuh"
 #include <stdlib.h>
+#include <type_traits>
 
 namespace fcb {
 
@@ -200,8 +201,10 @@ __global__ void __launch_bounds__(TcRoles<N_TILE>::THREADS, 1) conv1d_tc_kernel(
     double* red = reinterpret_cast<double*>(raw_empty + TC_RAW_MAX);   // [PARTS][8][2] statistics scratch + finalisation flag
     uint8_t* smR = smem_raw + L.off_raw;
     // TMA-staged units (nraw > 0, 1-D layers): an INTERIOR tile needs only rows inside [0, rows covered by the tensor map) -- no
-    // reflection, no zero padding -- so its units arrive as dense [a_rows][32 channel] boxes through the raw ring; the first / last
-    // tiles of a clip keep the per-thread global loads (the index map lives there).  Units of a tile in ring order:
+    // reflection, no zero padding -- so its units arrive as dense [a_rows][32 channel] boxes through the raw ring.  In a 1-D layer the
+    // first / last tiles of a clip take the ring too: the box zero-fills the rows outside the input, and the producers apply the
+    // per-thread path's index map to those rows (zero, or a reflected row read from global memory).  The 2-D mode keeps its edge
+    // tiles on the per-thread global loads.  Units of a tile in ring order:
     // stage-major, half-minor; every role derives the slot from the same running count.
 #define units_per_tile ka.units_per_tile
 #define tq_rows ka.tq_rows                  /* rows per phase the tensor map exposes */
@@ -214,6 +217,9 @@ __global__ void __launch_bounds__(TcRoles<N_TILE>::THREADS, 1) conv1d_tc_kernel(
         const int hi = t_last * S - p.pad_l + (K - 1);
         return lo >= 0 && hi < tq_rows * S;
     };
+    // tiles whose units come through the raw ring: every tile of a 1-D layer (an edge tile patches its padding rows per row, see the
+    // producers), the interior tiles of a 2-D layer
+    auto tile_raw = [&](int t0) -> bool { return FREQ ? tile_interior(t0) : nraw > 0; };
 
     if (tid == 0) {
         for (int i = 0; i < na_stages; ++i) { mbar_init(a_full + i, split ? 2 * TC_PROD : TC_PROD); mbar_init(a_empty + i, 2); }
@@ -248,7 +254,7 @@ __global__ void __launch_bounds__(TcRoles<N_TILE>::THREADS, 1) conv1d_tc_kernel(
         const float in_scale = p.tc_in_scale;
         int rawbase = 0;                            // raw-ring units of the interior tiles this CTA has passed
         while (unit >= n_units && tile < n_tiles) {
-            if (tile_interior(tc_tile(tile, n_nt, n_tt).tt * TC_M)) rawbase += units_per_tile;
+            if (tile_raw(tc_tile(tile, n_nt, n_tt).tt * TC_M)) rawbase += units_per_tile;
             unit -= n_units; tile += gridDim.x;
         }
         while (tile < n_tiles) {
@@ -262,7 +268,8 @@ __global__ void __launch_bounds__(TcRoles<N_TILE>::THREADS, 1) conv1d_tc_kernel(
             const float* cf0 = p.in0.coef ? p.in0.coef + (long long)b * 2 * pitch : nullptr;
             const float* cf1 = (has1 && p.in1.coef) ? p.in1.coef + (long long)b * 2 * pitch : nullptr;
             const int cur_tile = tile;
-            const bool interior = tile_interior(t0);
+            const bool raw = tile_raw(t0);
+            const bool edge = !FREQ && raw && !tile_interior(t0);   // raw-staged edge tile (1-D): padding rows patched per row
             for (; unit < n_units && tile == cur_tile; ) {
                 const int sc = unit / S, ph = unit - sc * S;
                 const int chunk = 2 * sc + half;               // 32-channel chunk of this group (may not exist: odd n_chunks)
@@ -274,7 +281,7 @@ __global__ void __launch_bounds__(TcRoles<N_TILE>::THREADS, 1) conv1d_tc_kernel(
                     if (p.dbg & 64) mbar_wait(a_empty + as, par); else mbar_wait_backoff(a_empty + as, par, 64);
                 } else if (chunk >= n_chunks) {
                     if (p.dbg & 64) mbar_wait(a_empty + as, par); else mbar_wait_backoff(a_empty + as, par, 64);      // missing half of the last stage: never read by the MMAs
-                } else if (interior) {
+                } else if (raw) {
                     // ---- TMA-staged unit: the dense [a_rows][32 ch] boxes (+ the coefficient slices) wait in the raw ring; rows go
                     // shared -> registers -> shared one at a time (no long-latency loads to batch, few live registers)
                     bool c_ok = chunk * TC_KC + jchunk * 4 < C_in;
@@ -303,34 +310,55 @@ __global__ void __launch_bounds__(TcRoles<N_TILE>::THREADS, 1) conv1d_tc_kernel(
                     }
                     if (p.dbg & 64) mbar_wait(a_empty + as, par); else mbar_wait_backoff(a_empty + as, par, 64);
                     const uint8_t* rrow = rb + rsub * raw_pitch + jchunk * 16;
-#pragma unroll
-                    for (int i = 0; i < NR; ++i) {
-                        const int u = rsub + TC_PROWS * i;
-                        if (u < L.a_rows) {
-                            float4 v = make_float4(0.f, 0.f, 0.f, 0.f);
-                            if (c_ok) {
-                                const float4 xv = *reinterpret_cast<const float4*>(rrow + i * TC_PROWS * raw_pitch);
-                                v.x = fmaf(xv.x, a0.x, b0.x); v.y = fmaf(xv.y, a0.y, b0.y);
-                                v.z = fmaf(xv.z, a0.z, b0.z); v.w = fmaf(xv.w, a0.w, b0.w);
-                                if (has1) {
-                                    const float4 yv = *reinterpret_cast<const float4*>(rrow + L.raw_in1 + i * TC_PROWS * raw_pitch);
-                                    v.x = v.x + fmaf(yv.x, a1.x, b1.x); v.y = v.y + fmaf(yv.y, a1.y, b1.y);
-                                    v.z = v.z + fmaf(yv.z, a1.z, b1.z); v.w = v.w + fmaf(yv.w, a1.w, b1.w);
+                    // edge tiles apply the index map per row; interior tiles compile without it
+                    auto raw_rows = [&](auto edge_c) {
+                        constexpr bool EDGE = decltype(edge_c)::value;
+                        constexpr int UNROLL = EDGE ? 1 : NR;  // the edge body, unrolled, does not fit the producer register budget
+#pragma unroll UNROLL
+                        for (int i = 0; i < NR; ++i) {
+                            const int u = rsub + TC_PROWS * i;
+                            if (u < L.a_rows) {
+                                float4 v = make_float4(0.f, 0.f, 0.f, 0.f);
+                                bool ok = c_ok, from_gl = false;
+                                long long goff = 0;
+                                if (EDGE) {
+                                    // the index map of the per-thread path: a zero row stays zero; a reflected row, or one the tensor map
+                                    // does not cover, is read from global memory; every other row is the box row
+                                    const int gt = (t0 + u) * S + ph - p.pad_l;
+                                    int src = gt;
+                                    ok = ok && gt <= gt_max;
+                                    if (p.pad_zero) ok = ok && gt >= 0 && gt < p.T_in;
+                                    else { src = reflect_index(gt, p.T_ext); ok = ok && src < p.T_in && src >= 0; }
+                                    from_gl = src != gt || gt >= tq_rows * S;
+                                    goff = (long long)src * C_in + chunk * TC_KC + jchunk * 4;
                                 }
-                                if (p.elu) {
-                                    v.x = elu_scaled(v.x, p.tc_elu_k, in_scale); v.y = elu_scaled(v.y, p.tc_elu_k, in_scale);
-                                    v.z = elu_scaled(v.z, p.tc_elu_k, in_scale); v.w = elu_scaled(v.w, p.tc_elu_k, in_scale);
+                                if (ok) {
+                                    const float4 xv = from_gl ? __ldg(reinterpret_cast<const float4*>(x0 + goff))
+                                                              : *reinterpret_cast<const float4*>(rrow + i * TC_PROWS * raw_pitch);
+                                    v.x = fmaf(xv.x, a0.x, b0.x); v.y = fmaf(xv.y, a0.y, b0.y);
+                                    v.z = fmaf(xv.z, a0.z, b0.z); v.w = fmaf(xv.w, a0.w, b0.w);
+                                    if (has1) {
+                                        const float4 yv = from_gl ? __ldg(reinterpret_cast<const float4*>(x1 + goff))
+                                                                  : *reinterpret_cast<const float4*>(rrow + L.raw_in1 + i * TC_PROWS * raw_pitch);
+                                        v.x = v.x + fmaf(yv.x, a1.x, b1.x); v.y = v.y + fmaf(yv.y, a1.y, b1.y);
+                                        v.z = v.z + fmaf(yv.z, a1.z, b1.z); v.w = v.w + fmaf(yv.w, a1.w, b1.w);
+                                    }
+                                    if (p.elu) {
+                                        v.x = elu_scaled(v.x, p.tc_elu_k, in_scale); v.y = elu_scaled(v.y, p.tc_elu_k, in_scale);
+                                        v.z = elu_scaled(v.z, p.tc_elu_k, in_scale); v.w = elu_scaled(v.w, p.tc_elu_k, in_scale);
+                                    }
                                 }
+                                if (p.dbg & 4) continue;
+                                uint2 h, l;
+                                split_f16x2(v.x, v.y, h.x, l.x);
+                                split_f16x2(v.z, v.w, h.y, l.y);
+                                const uint32_t o = (uint32_t)u * 128u + ((c16 ^ (uint32_t)(u & 7)) << 4) + sub8;
+                                *reinterpret_cast<uint2*>(hi + o) = h;
+                                *reinterpret_cast<uint2*>(lo + o) = l;
                             }
-                            if (p.dbg & 4) continue;
-                            uint2 h, l;
-                            split_f16x2(v.x, v.y, h.x, l.x);
-                            split_f16x2(v.z, v.w, h.y, l.y);
-                            const uint32_t o = (uint32_t)u * 128u + ((c16 ^ (uint32_t)(u & 7)) << 4) + sub8;
-                            *reinterpret_cast<uint2*>(hi + o) = h;
-                            *reinterpret_cast<uint2*>(lo + o) = l;
                         }
-                    }
+                    };
+                    if (edge) raw_rows(std::true_type{}); else raw_rows(std::false_type{});
                     mbar_arrive(raw_empty + rslot);            // the raw rows have been consumed
                     fence_proxy_async_smem();
                 } else {
@@ -430,7 +458,7 @@ __global__ void __launch_bounds__(TcRoles<N_TILE>::THREADS, 1) conv1d_tc_kernel(
                 unit += step;
             }
             while (unit >= n_units && tile < n_tiles) {
-                if (tile_interior(tc_tile(tile, n_nt, n_tt).tt * TC_M)) rawbase += units_per_tile;
+                if (tile_raw(tc_tile(tile, n_nt, n_tt).tt * TC_M)) rawbase += units_per_tile;
                 unit -= n_units; tile += gridDim.x;
             }
         }
@@ -472,7 +500,7 @@ __global__ void __launch_bounds__(TcRoles<N_TILE>::THREADS, 1) conv1d_tc_kernel(
             for (int tile = blockIdx.x; tile < n_tiles; tile += gridDim.x) {
                 const TcTile tl = tc_tile(tile, n_nt, n_tt);
                 const int t0 = tl.tt * TC_M;
-                if (!tile_interior(t0)) continue;
+                if (!tile_raw(t0)) continue;
                 int b = tl.b, f_out = 0;
                 if (FREQ) { b = tl.b / p.fq.F_out; f_out = tl.b - b * p.fq.F_out; }
                 const int pitch = FREQ ? p.fq.cin : C_in;
@@ -911,11 +939,12 @@ cudaError_t launch_conv_tc(const ConvParams& p_in, int B, cudaStream_t st, int* 
     *nparts = n_tt * (p.C_out / tc_part_cols(p.C_out));
     const int n_tiles = n_tt * n_nt * B;
     const bool freq = p.fq.KF > 0;          // B counts pseudo-clips (clips x output frequency rows) in the 2-D mode
-    // raw TMA ring: 1-D layers with interior tiles (n_tt >= 3), channel counts the box covers, 16-byte aligned views
+    // raw TMA ring: every 1-D layer (edge tiles included) and the 2-D layers with interior tiles, channel counts the box covers,
+    // 16-byte aligned views
     CUtensorMap tm0{}, tm1{};
     // (2-D: a 32-channel unit must be a slice of ONE frequency tap -> cin % 32 == 0, or the single tap of a 16-channel 1x1 conv)
-    // (interior tiles exist when the clip has at least 3 tiles, or for 1x1 layers -- no halo -- always)
-    bool want_raw = g_tma_state == 1 && (n_tt >= 3 || (p.K == 1 && p.S == 1 && p.pad_l == 0)) && p.T_in / p.S >= 1 &&
+    // (2-D: interior tiles exist when the clip has at least 3 tiles, or for 1x1 layers -- no halo -- always)
+    bool want_raw = g_tma_state == 1 && (!freq || n_tt >= 3 || (p.K == 1 && p.S == 1 && p.pad_l == 0)) && p.T_in / p.S >= 1 &&
                     (freq ? (p.fq.cin % TC_KC == 0 || (p.fq.cin == 16 && p.fq.KF == 1)) : (p.C_in % TC_KC == 0 || p.C_in == 16));
     // 2-D layers: built and parity-tested (5-D tensor maps) but opt-in (FCB_TC_TMA2D=1): the K_F-fold re-read of every input row
     // makes the unit stream L2-bound either way and the TMA path adds a hand-off
