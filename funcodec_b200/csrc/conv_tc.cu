@@ -32,6 +32,10 @@
 //   * N_TILE = 128 (1-D layers with C_out % 128 == 0) transforms each activation element once per 128 output columns instead
 //     of once per 64; its epilogue still writes one GroupNorm partial per 64 columns, at the index a 64-column tile would
 //     use, so the statistics (and every output bit) do not depend on the tile width.
+//   * 2-CTA pairs (PAIR, 1-D N_TILE = 128 layers on the raw ring with an even number of n-tiles): a cluster's two CTAs take
+//     n-tiles 2j and 2j + 1 of one time tile, whose A stages are identical.  Each fetches and transforms half of the slab rows and
+//     copies them into the peer's stage (cp.async.bulk shared::cta -> shared::cluster, completing on the peer's a_full); each
+//     consumer warpgroup releases a stage in both CTAs.  Weights, MMA issue and epilogue are those of the single-CTA kernel.
 //   * the tensor core adds into its fp32 accumulator with truncation, so a long chain loses ~1 ulp per MMA:
 //     chains are cut every ~48 MMAs and each finished group is folded into running totals (registers) with
 //     round-to-nearest CUDA-core adds; the epilogue (bias, channels-last store, GroupNorm partial sums) reads the totals.
@@ -102,19 +106,24 @@ struct TcSmemLayout {
     int off_b, off_raw, off_bar, total;
 };
 
+// A slab rows a CTA transforms and its raw boxes hold: all a_rows, or in a 2-CTA pair the share of rank 0 (rows [0, share)), rank 1
+// taking the rest; a multiple of 8 rows keeps both shares whole swizzle groups
+__host__ __device__ inline int tc_raw_rows(int a_rows, bool pair) { return pair ? ((a_rows / 2 + 7) / 8) * 8 : a_rows; }
+
 __host__ __device__ inline TcSmemLayout tc_layout(int K, int S, int n_tile, int na, int nb, int nraw = 0, int raw_pitch = 128,
-                                                   int has1 = 0) {
+                                                   int has1 = 0, bool pair = false) {
     TcSmemLayout L;
     const int qmax = (K - 1) / S;
     L.a_rows = ((TC_M + qmax + 7) / 8) * 8;
+    const int raw_rows = tc_raw_rows(L.a_rows, pair);
     L.a_stage = 2 * L.a_rows * 128;
     L.b_stage = 2 * n_tile * 128;
     L.na = na; L.nb = nb;
     L.off_b = na * L.a_stage;
     // raw slot: [in0 rows][in1 rows][a0 | b0 | a1 | b1 coefficient slices of the unit's 32 channels (4 x 128 B)]
     L.nraw = nraw;
-    L.raw_in1 = L.a_rows * raw_pitch;
-    L.raw_cf = (1 + has1) * L.a_rows * raw_pitch;
+    L.raw_in1 = raw_rows * raw_pitch;
+    L.raw_cf = (1 + has1) * raw_rows * raw_pitch;
     L.raw_slot = (L.raw_cf + 512 + 127) / 128 * 128;
     L.off_raw = L.off_b + nb * L.b_stage;
     L.off_bar = L.off_raw + nraw * L.raw_slot;
@@ -136,6 +145,7 @@ struct TcArgs {
     TcSmemLayout L;
     int na, nb, n_tiles, w_resident, nraw;
     int n_chunks, n_sc, split, n_units, upg, n_groups, n_tt, n_nt, units_per_tile, tq_rows, raw_pitch;
+    int raw_rows;      // tc_raw_rows
 };
 
 struct TcTile { int b, nt, tt; };
@@ -164,10 +174,15 @@ __device__ __forceinline__ void tc_issue_tap(float (&acc)[N_TILE / 2], uint32_t 
     wgmma_commit();
 }
 
-template <int N_TILE, bool FREQ>
+// PAIR (1-D, N_TILE = 128, raw ring, an even number of n-tiles; launched as 2-CTA clusters): the CTAs of a cluster take n-tiles
+// 2j and 2j + 1 of the same (clip, time tile) -- the tile list puts n-tiles fastest and the grid is even, so the usual walk
+// (blockIdx.x, stride gridDim.x) gives them that pairing at every step.  Their A stages are identical: cluster rank r fetches and
+// transforms only its share of the slab rows (ka.raw_rows rows from r * ka.raw_rows) and copies them into the peer's stage.
+template <int N_TILE, bool FREQ, bool PAIR = false>
 __global__ void __launch_bounds__(TcRoles<N_TILE>::THREADS, 1) conv1d_tc_kernel(const __grid_constant__ ConvParams p, const __grid_constant__ TcArgs ka,
                                                                  const __grid_constant__ CUtensorMap tm0,
                                                                  const __grid_constant__ CUtensorMap tm1) {
+    static_assert(!PAIR || (N_TILE == 128 && !FREQ), "pairs are built for the 1-D 128-column layout");
     using R = TcRoles<N_TILE>;
     extern __shared__ __align__(1024) uint8_t smem_raw[];
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
@@ -221,13 +236,22 @@ __global__ void __launch_bounds__(TcRoles<N_TILE>::THREADS, 1) conv1d_tc_kernel(
     // producers), the interior tiles of a 2-D layer
     auto tile_raw = [&](int t0) -> bool { return FREQ ? tile_interior(t0) : nraw > 0; };
 
+    // PAIR: a_full also takes one local arrival that posts the expect_tx of the rows the peer copies in; a_empty takes both CTAs'
+    // consumer warpgroups, since a producer writes into both CTAs' stages
+    const uint32_t rank = PAIR ? cluster_ctarank() : 0u, peer = rank ^ 1u;
+    const int r0 = (int)rank * ka.raw_rows;                                         // first A slab row this CTA transforms
+    const int r_end = PAIR ? min(L.a_rows, r0 + ka.raw_rows) : L.a_rows;
     if (tid == 0) {
-        for (int i = 0; i < na_stages; ++i) { mbar_init(a_full + i, split ? 2 * TC_PROD : TC_PROD); mbar_init(a_empty + i, 2); }
+        for (int i = 0; i < na_stages; ++i) {
+            mbar_init(a_full + i, (split ? 2 * TC_PROD : TC_PROD) + (PAIR ? 1 : 0));
+            mbar_init(a_empty + i, PAIR ? 4 : 2);
+        }
         for (int i = 0; i < nb_stages; ++i) { mbar_init(b_full + i, 1); mbar_init(b_empty + i, 2); }
         for (int i = 0; i < TC_RAW_MAX; ++i) { mbar_init(raw_full + i, 1); mbar_init(raw_empty + i, TC_PROD); }
         mbar_fence_init();
     }
-    __syncthreads();
+    // PAIR: no remote arrival or copy may reach a barrier of the peer before the peer has initialised it
+    if (PAIR) cluster_sync(); else __syncthreads();
 
     const int role = warp >> 2;                     // warpgroup: producers, then control, then the two consumers
     if (role < R::PROD_GROUPS) {
@@ -240,6 +264,19 @@ __global__ void __launch_bounds__(TcRoles<N_TILE>::THREADS, 1) conv1d_tc_kernel(
         const int wq = (ptid >> 5), lq = (lane >> 3);
         const int rsub = ((wq >> 1) << 3) + ((wq & 1) << 1) + (lq & 1) + ((lq >> 1) << 2);      // TC_PROWS = 16 rows per pass
         constexpr int NR = TC_A_ROWS_MAX / TC_PROWS;                                             // passes per unit
+        // passes per raw unit: a PAIR CTA transforms at most half of the rows, rounded up to 8
+        constexpr int NR_RAW = PAIR ? ((TC_A_ROWS_MAX / 2 + 7) / 8 * 8 + TC_PROWS - 1) / TC_PROWS : NR;
+        auto wait_a_empty = [&](uint64_t* bar, uint32_t par) {
+            if (PAIR) mbar_wait_cluster_backoff(bar, par, 64);       // the peer's consumers arrive on it too
+            else if (p.dbg & 64) mbar_wait(bar, par);
+            else mbar_wait_backoff(bar, par, 64);
+        };
+        // PAIR hand-off: this CTA's rows of the hi and lo slabs go to the same offsets in the peer's stage (the swizzle follows the
+        // address, so a same-offset copy keeps the layout), completing on the peer's a_full
+        const uint32_t hand_bytes = (uint32_t)(r_end - r0) * 128u;
+        const uint32_t peer_bytes = 2u * (uint32_t)(L.a_rows - (r_end - r0)) * 128u;
+        const uint32_t smA_peer = PAIR ? mapa_shared(smem_u32(smA), peer) : 0u;
+        const uint32_t a_full_peer = PAIR ? mapa_shared(smem_u32(a_full), peer) : 0u;
         const int gt_max = (p.T_out - 1) * S - p.pad_l + (K - 1);
         // this group's cursor over the CTA's global stage sequence (tile-major).  split: every stage is filled by both groups
         // (group g writes the 32-channel half g), or by the single group, half 0 then half 1; otherwise (one 32-channel chunk)
@@ -278,10 +315,10 @@ __global__ void __launch_bounds__(TcRoles<N_TILE>::THREADS, 1) conv1d_tc_kernel(
                 uint8_t* lo = hi + L.a_rows * 128;
                 const uint32_t c16 = (uint32_t)(half * 4 + (jchunk >> 1)), sub8 = (uint32_t)((jchunk & 1) << 3);
                 if (p.dbg & 512) {
-                    if (p.dbg & 64) mbar_wait(a_empty + as, par); else mbar_wait_backoff(a_empty + as, par, 64);
+                    wait_a_empty(a_empty + as, par);
                 } else if (chunk >= n_chunks) {
-                    if (p.dbg & 64) mbar_wait(a_empty + as, par); else mbar_wait_backoff(a_empty + as, par, 64);      // missing half of the last stage: never read by the MMAs
-                } else if (raw) {
+                    wait_a_empty(a_empty + as, par);      // missing half of the last stage: never read by the MMAs
+                } else if (PAIR || raw) {
                     // ---- TMA-staged unit: the dense [a_rows][32 ch] boxes (+ the coefficient slices) wait in the raw ring; rows go
                     // shared -> registers -> shared one at a time (no long-latency loads to batch, few live registers)
                     bool c_ok = chunk * TC_KC + jchunk * 4 < C_in;
@@ -308,16 +345,16 @@ __global__ void __launch_bounds__(TcRoles<N_TILE>::THREADS, 1) conv1d_tc_kernel(
                             b1.x *= in_scale; b1.y *= in_scale; b1.z *= in_scale; b1.w *= in_scale;
                         }
                     }
-                    if (p.dbg & 64) mbar_wait(a_empty + as, par); else mbar_wait_backoff(a_empty + as, par, 64);
+                    wait_a_empty(a_empty + as, par);
                     const uint8_t* rrow = rb + rsub * raw_pitch + jchunk * 16;
                     // edge tiles apply the index map per row; interior tiles compile without it
                     auto raw_rows = [&](auto edge_c) {
                         constexpr bool EDGE = decltype(edge_c)::value;
                         constexpr int UNROLL = EDGE ? 1 : NR;  // the edge body, unrolled, does not fit the producer register budget
 #pragma unroll UNROLL
-                        for (int i = 0; i < NR; ++i) {
-                            const int u = rsub + TC_PROWS * i;
-                            if (u < L.a_rows) {
+                        for (int i = 0; i < NR_RAW; ++i) {
+                            const int u = r0 + rsub + TC_PROWS * i;
+                            if (u < r_end) {
                                 float4 v = make_float4(0.f, 0.f, 0.f, 0.f);
                                 bool ok = c_ok, from_gl = false;
                                 long long goff = 0;
@@ -416,7 +453,7 @@ __global__ void __launch_bounds__(TcRoles<N_TILE>::THREADS, 1) conv1d_tc_kernel(
                         }
                     }
                     if (i0 == 0) {
-                        if (p.dbg & 64) mbar_wait(a_empty + as, par); else mbar_wait_backoff(a_empty + as, par, 64);
+                        wait_a_empty(a_empty + as, par);
                     }
 #pragma unroll
                     for (int j = 0; j < PB; ++j) {
@@ -452,6 +489,20 @@ __global__ void __launch_bounds__(TcRoles<N_TILE>::THREADS, 1) conv1d_tc_kernel(
                 }
                 mbar_arrive(a_full + as);
                 if (R::PROD_GROUPS == 1 && split && half == 0) { half = 1; continue; }   // the stage's second half
+                if (PAIR) {
+                    // every producer thread has fenced its stores to the async proxy; one thread then copies the rows to the peer
+                    // and posts, with the one extra local arrival, the bytes the peer copies into this stage (a peer copy that
+                    // completes first only drives the tx-count below zero: the pending arrival keeps the phase open).  The source
+                    // rows are not overwritten before the copy has read them: the next write of this stage waits for a_empty,
+                    // which the peer's consumers arrive on only after the peer's a_full -- and so this copy -- has completed.
+                    asm volatile("bar.sync 2, 128;" ::: "memory");
+                    if (ptid == 0) {
+                        const uint32_t so = (uint32_t)(as * L.a_stage + r0 * 128);
+                        bulk_s2peer(smA_peer + so, smA + so, hand_bytes, a_full_peer + 8u * (uint32_t)as);
+                        bulk_s2peer(smA_peer + so + L.a_rows * 128, smA + so + L.a_rows * 128, hand_bytes, a_full_peer + 8u * (uint32_t)as);
+                        mbar_arrive_expect_tx(a_full + as, peer_bytes);
+                    }
+                }
                 half = half0;
                 as += step;
                 if (as >= na_stages) { as -= na_stages; aphase ^= 1; }
@@ -492,7 +543,7 @@ __global__ void __launch_bounds__(TcRoles<N_TILE>::THREADS, 1) conv1d_tc_kernel(
             }
         } else if (warp == 4 * R::CTL_WG + 1 && lane == 0 && nraw > 0 && !(p.dbg & 512)) {
             // raw activation tiles via TMA (cp.async.bulk.tensor)
-            const uint32_t row_bytes = (uint32_t)(L.a_rows * raw_pitch);
+            const uint32_t row_bytes = (uint32_t)(ka.raw_rows * raw_pitch);   // the box: this CTA's share of the slab rows
             const uint32_t cbytes = (uint32_t)raw_pitch;
             const uint32_t n_cf = (p.in0.coef ? 2u : 0u) + ((has1 && p.in1.coef) ? 2u : 0u);
             const uint32_t unit_bytes = row_bytes * (has1 ? 2u : 1u) + n_cf * cbytes;
@@ -530,8 +581,8 @@ __global__ void __launch_bounds__(TcRoles<N_TILE>::THREADS, 1) conv1d_tc_kernel(
                                 tma_load_5d(dst, &tm0, c0, php, tq0, f_src, b, raw_full + slot);
                                 if (has1) tma_load_5d(dst + L.raw_in1, &tm1, c0, php, tq0, f_src, b, raw_full + slot);
                             } else {
-                                tma_load_4d(dst, &tm0, c0, php, tq0, b, raw_full + slot);
-                                if (has1) tma_load_4d(dst + L.raw_in1, &tm1, c0, php, tq0, b, raw_full + slot);
+                                tma_load_4d(dst, &tm0, c0, php, tq0 + r0, b, raw_full + slot);
+                                if (has1) tma_load_4d(dst + L.raw_in1, &tm1, c0, php, tq0 + r0, b, raw_full + slot);
                             }
                             if (cf0) {
                                 bulk_g2s(dst + L.raw_cf, cf0 + c0, cbytes, raw_full + slot);
@@ -556,6 +607,7 @@ __global__ void __launch_bounds__(TcRoles<N_TILE>::THREADS, 1) conv1d_tc_kernel(
         const int ctid = tid - 128 * R::CONS_WG;                  // 0..255
         const bool leader = (tid & 127) == 0;                     // one arrival per warpgroup on the ring barriers
         const uint32_t a_base = smem_u32(smA) + (uint32_t)(wg * 64 * 128), b_base = smem_u32(smB);
+        const uint32_t a_empty_peer = PAIR ? mapa_shared(smem_u32(a_empty), peer) : 0u;   // PAIR: the peer wrote rows of our stages
         const int r_lo = wg * 64 + (cw & 3) * 16 + (lane >> 2);   // accumulator rows of this thread: r_lo, r_lo + 8
         const int cq = 2 * (lane & 3);                            // first of its two columns in every 8-column group
         // 2-D plain convs (no phase scatter, no padded columns) store [pseudo-clip][t][C_out] like a 1-D layer
@@ -642,6 +694,7 @@ __global__ void __launch_bounds__(TcRoles<N_TILE>::THREADS, 1) conv1d_tc_kernel(
                         // the previous tap's commit group has completed: release what only it read (predicated, no branch)
                         mbar_arrive_if(b_empty + pend_b, leader && pend_b >= 0);
                         mbar_arrive_if(a_empty + pend_a, leader && pend_a >= 0);
+                        if (PAIR) mbar_arrive_remote_if(a_empty_peer + 8u * (uint32_t)pend_a, leader && pend_a >= 0);
                         pend_b = w_resident ? -1 : bs;
                         pend_a = -1;
                         if (++bs == nb_stages) { bs = 0; bphase ^= 1; }
@@ -655,6 +708,7 @@ __global__ void __launch_bounds__(TcRoles<N_TILE>::THREADS, 1) conv1d_tc_kernel(
                 if (leader) {
                     if (pend_b >= 0) mbar_arrive(b_empty + pend_b);
                     if (pend_a >= 0) mbar_arrive(a_empty + pend_a);
+                    if (PAIR && pend_a >= 0) mbar_arrive_remote_if(a_empty_peer + 8u * (uint32_t)pend_a, true);
                 }
                 pend_a = -1; pend_b = -1;
 #pragma unroll
@@ -742,6 +796,8 @@ __global__ void __launch_bounds__(TcRoles<N_TILE>::THREADS, 1) conv1d_tc_kernel(
         }
         if (p.fin_counter && p.partials && !(p.dbg & 16)) fin_flush();
     }
+    // PAIR: no CTA exits while its peer can still copy into its shared memory or arrive on its barriers
+    if (PAIR) cluster_sync();
 #undef na_stages
 #undef nb_stages
 #undef n_tiles
@@ -800,7 +856,15 @@ struct TcPlan { int resident, na, nb, nraw; TcSmemLayout L; bool ok; };
 // issue, so 2 stages suffice and the rest of the shared memory buys prefetch depth (nraw units in flight).
 // At N_TILE = 128 a B stage is 32 KB; the last fallback (na = nb = 2) still fits every supported shape: A 2 x 36 KB (144 rows)
 // + B 2 x 32 KB + two raw slots of a two-input unit (2 x 36.5 KB) + barriers and scratch = 209.5 KB of 225.
-static TcPlan tc_plan(const ConvParams& p, int na_first, bool want_raw, int g_deep_ring) {
+// pair: the raw slots hold a 2-CTA pair's share of the slab rows (tc_layout), so they are half as large.  A pair asks for 3 A stages
+// first: the copy to the peer and the release by both CTAs' consumers lengthen a stage's round trip, and with 2 stages the 1-tap
+// layers lose more to that than they gain from the halved transform.  A pair whose stages feed two taps (the 8/4, 10/5 and 16/8 down
+// convs, the up convs) asks for 2 B stages first, which leaves room for a deeper raw ring; with more taps per stage the B ring stays
+// deeper (the k7 `dec.conv0` was 16 % slower at 2 B stages).  What the fallbacks below give, per (taps per stage, inputs):
+//   1 tap,  one input:  na 3, nb 3, nraw 3      1 tap,  two inputs:  na 2, nb 3, nraw 3  (na 3 leaves no room for two raw slots)
+//   2 taps, one input:  na 3, nb 2, nraw 6      2 taps, two inputs:  na 3, nb 2, nraw 3
+//   3+ taps, one input: na 3, nb 3, nraw 2      3+ taps, two inputs: na 2, nb 3, nraw 3
+static TcPlan tc_plan(const ConvParams& p, int na_first, bool want_raw, int g_deep_ring, bool pair = false) {
     const int limit = 225 * 1024;
     const int n_slabs = ((p.C_in + 2 * TC_KC - 1) / (2 * TC_KC)) * p.K;   // (64-channel stage chunk, tap) weight slabs per n-tile
     const int has1 = p.in1.x ? 1 : 0;
@@ -808,10 +872,10 @@ static TcPlan tc_plan(const ConvParams& p, int na_first, bool want_raw, int g_de
     const int raw_pitch = (cin_row < TC_KC ? cin_row : TC_KC) * 4;
     TcPlan pl{};
     pl.ok = false;
-    int na = na_first, nb = 4;
+    int na = pair ? 3 : na_first, nb = (pair && (p.K + p.S - 1) / p.S == 2) ? 2 : 4;
     TcSmemLayout L = tc_layout(p.K, p.S, p.n_tile, na, n_slabs);
     const int min_raw = want_raw ? 2 : 0;
-    auto fits = [&](const TcSmemLayout& l) { return l.total + min_raw * tc_layout(p.K, p.S, p.n_tile, 2, 2, 1, raw_pitch, has1).raw_slot <= limit; };
+    auto fits = [&](const TcSmemLayout& l) { return l.total + min_raw * tc_layout(p.K, p.S, p.n_tile, 2, 2, 1, raw_pitch, has1, pair).raw_slot <= limit; };
     if (n_slabs <= 64 && p.C_out == p.n_tile && fits(L)) { pl.resident = 1; nb = n_slabs; }   // one n-tile only
     else {
         L = tc_layout(p.K, p.S, p.n_tile, na, nb);
@@ -828,9 +892,9 @@ static TcPlan tc_plan(const ConvParams& p, int na_first, bool want_raw, int g_de
     int nraw = 0;
     if (want_raw) {
         nraw = 2;
-        while (nraw < TC_RAW_MAX && tc_layout(p.K, p.S, p.n_tile, na, nb, nraw + 1, raw_pitch, has1).total <= limit) ++nraw;
+        while (nraw < TC_RAW_MAX && tc_layout(p.K, p.S, p.n_tile, na, nb, nraw + 1, raw_pitch, has1, pair).total <= limit) ++nraw;
     }
-    pl.L = tc_layout(p.K, p.S, p.n_tile, na, nb, nraw, raw_pitch, has1);
+    pl.L = tc_layout(p.K, p.S, p.n_tile, na, nb, nraw, raw_pitch, has1, pair);
     pl.na = na; pl.nb = nb; pl.nraw = nraw;
     pl.ok = pl.L.total <= limit;
     return pl;
@@ -872,10 +936,15 @@ static bool make_act_map_2d(CUtensorMap* tm, const InView& v, int cin, int ST, i
                           CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) == CUDA_SUCCESS;
 }
 
-template <int N_TILE, bool FREQ>
+// 2-CTA clusters of the PAIR kernel a device holds at once (at 225 KB of shared memory each), per device ordinal: a process may
+// drive devices of different models (ordinals beyond the table are queried at every launch)
+constexpr int TC_PAIR_DEVICES = 64;
+static int g_max_pairs[TC_PAIR_DEVICES] = {};
+
+template <int N_TILE, bool FREQ, bool PAIR = false>
 static cudaError_t launch_tc_n(const ConvParams& p, cudaStream_t st, const TcPlan& pl, int n_tiles, const CUtensorMap& tm0,
                                const CUtensorMap& tm1) {
-    auto kern = conv1d_tc_kernel<N_TILE, FREQ>;
+    auto kern = conv1d_tc_kernel<N_TILE, FREQ, PAIR>;
     {
         cudaError_t e = ensure_dynamic_smem((const void*)kern, 225 * 1024);
         if (e != cudaSuccess) return e;
@@ -894,6 +963,37 @@ static cudaError_t launch_tc_n(const ConvParams& p, cudaStream_t st, const TcPla
     ka.units_per_tile = ka.n_chunks * p.S;
     ka.tq_rows = p.T_in / p.S;
     ka.raw_pitch = ((FREQ ? p.fq.cin : p.C_in) < TC_KC ? (FREQ ? p.fq.cin : p.C_in) : TC_KC) * 4;
+    ka.raw_rows = tc_raw_rows(pl.L.a_rows, PAIR);
+    if (PAIR) {
+        cudaLaunchAttribute attr[1];
+        attr[0].id = cudaLaunchAttributeClusterDimension;
+        attr[0].val.clusterDim.x = 2; attr[0].val.clusterDim.y = 1; attr[0].val.clusterDim.z = 1;
+        cudaLaunchConfig_t cfg = {};
+        cfg.blockDim = dim3(TcRoles<N_TILE>::THREADS);
+        cfg.stream = st;
+        cfg.attrs = attr;
+        cfg.numAttrs = 1;
+        int dev = 0;
+        cudaError_t e = cudaGetDevice(&dev);
+        if (e != cudaSuccess) return e;
+        int max_pairs = dev < TC_PAIR_DEVICES ? g_max_pairs[dev] : 0;
+        if (max_pairs == 0) {
+            int sms = 0;
+            e = cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
+            if (e != cudaSuccess) return e;
+            cfg.gridDim = dim3(sms / 2 * 2);
+            cfg.dynamicSmemBytes = 225 * 1024;
+            e = cudaOccupancyMaxActiveClusters(&max_pairs, kern, &cfg);
+            if (e != cudaSuccess) return e;
+            if (max_pairs < 1) return cudaErrorInvalidConfiguration;
+            if (dev < TC_PAIR_DEVICES) g_max_pairs[dev] = max_pairs;
+        }
+        // n_tiles is even (an even number of n-tiles per time tile), so both CTAs of a cluster walk the same number of tiles
+        const int pairs = n_tiles / 2 < max_pairs ? n_tiles / 2 : max_pairs;
+        cfg.gridDim = dim3(2 * pairs);
+        cfg.dynamicSmemBytes = pl.L.total;
+        return cudaLaunchKernelEx(&cfg, kern, p, ka, tm0, tm1);
+    }
     kern<<<grid, TcRoles<N_TILE>::THREADS, pl.L.total, st>>>(p, ka, tm0, tm1);
     return cudaGetLastError();
 }
@@ -949,13 +1049,16 @@ cudaError_t launch_conv_tc(const ConvParams& p_in, int B, cudaStream_t st, int* 
     // 2-D layers: built and parity-tested (5-D tensor maps) but opt-in (FCB_TC_TMA2D=1): the K_F-fold re-read of every input row
     // makes the unit stream L2-bound either way and the TMA path adds a hand-off
     if (freq && !(getenv("FCB_TC_TMA2D") && atoi(getenv("FCB_TC_TMA2D")) != 0)) want_raw = false;
+    // 2-CTA pairs (conv1d_tc_kernel<128, false, true>): 1-D 128-column layers on the raw ring with an even number of n-tiles, whose
+    // CTAs would otherwise each fetch and transform the same activation rows
+    const bool pair = !freq && p.n_tile == 128 && n_nt % 2 == 0;
     TcPlan pl{};
     if (want_raw) {
-        pl = tc_plan(p, g_na_tma, true, g_deep_ring);
+        pl = tc_plan(p, g_na_tma, true, g_deep_ring, pair);
         want_raw = pl.ok && pl.nraw >= 2;
         if (want_raw && !freq)
-            want_raw = make_act_map(&tm0, p.in0, p.C_in, p.S, p.T_in, B, pl.L.a_rows) &&
-                       (!p.in1.x || make_act_map(&tm1, p.in1, p.C_in, p.S, p.T_in, B, pl.L.a_rows));
+            want_raw = make_act_map(&tm0, p.in0, p.C_in, p.S, p.T_in, B, tc_raw_rows(pl.L.a_rows, pair)) &&
+                       (!p.in1.x || make_act_map(&tm1, p.in1, p.C_in, p.S, p.T_in, B, tc_raw_rows(pl.L.a_rows, pair)));
         if (want_raw && freq) {
             const int nclips = B / p.fq.F_out;
             want_raw = make_act_map_2d(&tm0, p.in0, p.fq.cin, p.S, p.T_in, p.fq.F_in, p.fq.T_raw0, p.fq.f_off0, nclips, pl.L.a_rows) &&
@@ -970,7 +1073,10 @@ cudaError_t launch_conv_tc(const ConvParams& p_in, int B, cudaStream_t st, int* 
         case 16: return launch_tc_modes<16>(p, st, pl, n_tiles, freq, tm0, tm1);
         case 32: return launch_tc_modes<32>(p, st, pl, n_tiles, freq, tm0, tm1);
         case 64: return launch_tc_modes<64>(p, st, pl, n_tiles, freq, tm0, tm1);
-        case 128: return freq ? cudaErrorInvalidConfiguration : launch_tc_n<128, false>(p, st, pl, n_tiles, tm0, tm1);
+        case 128:
+            if (freq) return cudaErrorInvalidConfiguration;
+            return (pair && want_raw) ? launch_tc_n<128, false, true>(p, st, pl, n_tiles, tm0, tm1)
+                                      : launch_tc_n<128, false>(p, st, pl, n_tiles, tm0, tm1);
         default: return cudaErrorInvalidConfiguration;
     }
 }

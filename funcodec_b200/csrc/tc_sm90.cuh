@@ -52,8 +52,57 @@ __device__ __forceinline__ void mbar_wait_backoff(uint64_t* bar, uint32_t parity
     while (!mbar_try_wait(bar, parity)) { __nanosleep(ns); }
 }
 
+// Same, with cluster-scope acquire: for a barrier that the peer CTA of a cluster arrives on, so that the waiter's later writes
+// into the peer's shared memory are ordered after the peer's reads that preceded its arrival.
+__device__ __forceinline__ void mbar_wait_cluster_backoff(uint64_t* bar, uint32_t parity, unsigned ns) {
+    for (;;) {
+        uint32_t ok;
+        asm volatile(
+            "{\n\t.reg .pred p;\n\t"
+            "mbarrier.try_wait.parity.acquire.cluster.shared::cta.b64 p, [%1], %2;\n\t"
+            "selp.u32 %0, 1, 0, p;\n\t}"
+            : "=r"(ok)
+            : "r"(smem_u32(bar)), "r"(parity)
+            : "memory");
+        if (ok) return;
+        __nanosleep(ns);
+    }
+}
+
 // generic-proxy writes (st.shared by threads) -> visible to the async proxy (wgmma / bulk copies)
 __device__ __forceinline__ void fence_proxy_async_smem() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
+
+// ------------------------------------------------------------------------------------------------ thread-block clusters
+__device__ __forceinline__ uint32_t cluster_ctarank() {
+    uint32_t r;
+    asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r));
+    return r;
+}
+// shared::cluster address of the same shared-memory offset in CTA `rank` of the cluster
+__device__ __forceinline__ uint32_t mapa_shared(uint32_t smem_addr, uint32_t rank) {
+    uint32_t r;
+    asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(r) : "r"(smem_addr), "r"(rank));
+    return r;
+}
+// arrival on an mbarrier of another CTA of the cluster (`remote_bar`: from mapa_shared), by the threads whose `pred` is set, as a
+// predicated instruction (usable between wgmma of one warpgroup)
+__device__ __forceinline__ void mbar_arrive_remote_if(uint32_t remote_bar, bool pred) {
+    asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %1, 0;\n\t@p mbarrier.arrive.release.cluster.shared::cluster.b64 _, [%0];\n\t}" ::"r"(
+                     remote_bar),
+                 "r"((uint32_t)pred)
+                 : "memory");
+}
+// this CTA's shared memory -> the same-sized region of another CTA of the cluster (`dst_remote`, `bar_remote`: from mapa_shared),
+// completion signalled on that CTA's mbarrier (complete_tx::bytes).  16-byte aligned, size % 16 == 0.
+__device__ __forceinline__ void bulk_s2peer(uint32_t dst_remote, const void* src_smem, uint32_t bytes, uint32_t bar_remote) {
+    asm volatile("cp.async.bulk.shared::cluster.shared::cta.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];" ::"r"(dst_remote),
+                 "r"(smem_u32(src_smem)), "r"(bytes), "r"(bar_remote)
+                 : "memory");
+}
+// barrier over every thread of every CTA of the cluster (not .aligned: the roles reach it from divergent code)
+__device__ __forceinline__ void cluster_sync() {
+    asm volatile("barrier.cluster.arrive.release;\n\tbarrier.cluster.wait.acquire;" ::: "memory");
+}
 
 // ------------------------------------------------------------------------------------------------ bulk copy (TMA engine, 1-D)
 // global -> shared, completion signalled on an mbarrier (complete_tx::bytes).  16-byte aligned, size % 16 == 0.
