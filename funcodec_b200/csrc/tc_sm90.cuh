@@ -78,6 +78,12 @@ __device__ __forceinline__ uint32_t cluster_ctarank() {
     asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r));
     return r;
 }
+// CTAs in this CTA's cluster (1 for a launch without clusters)
+__device__ __forceinline__ uint32_t cluster_nctarank() {
+    uint32_t r;
+    asm volatile("mov.u32 %0, %%cluster_nctarank;" : "=r"(r));
+    return r;
+}
 // shared::cluster address of the same shared-memory offset in CTA `rank` of the cluster
 __device__ __forceinline__ uint32_t mapa_shared(uint32_t smem_addr, uint32_t rank) {
     uint32_t r;
