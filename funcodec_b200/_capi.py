@@ -27,6 +27,7 @@ class FcbConfig(Structure):
 
 
 FCB_MAX_TAIL_SEGMENTS = 16
+FCB_STREAM_ENCODE, FCB_STREAM_DECODE = 0, 1
 
 
 class FcbSegmentPlan(Structure):
@@ -68,6 +69,13 @@ SYMBOLS = {
                                           c_void_p, c_void_p, c_void_p, c_void_p]),
     "fcb_debug_conv2d": (c_int32, [c_void_p, c_char_p, c_void_p, c_int32, c_int32, c_int32, c_int32, c_void_p, c_int64, c_void_p,
                                    POINTER(c_int32), c_void_p]),
+    "fcb_stream_min_first_frames": (c_int32, [c_void_p]),
+    "fcb_stream_create": (c_int32, [c_void_p, c_int32, c_int32, c_void_p, POINTER(c_void_p)]),
+    "fcb_stream_encode": (c_int32, [c_void_p, c_void_p, c_int32, c_int32, c_void_p, c_void_p, c_void_p]),
+    "fcb_stream_decode_codes": (c_int32, [c_void_p, c_void_p, c_int32, c_int32, c_void_p, c_void_p]),
+    "fcb_stream_decode_emb": (c_int32, [c_void_p, c_void_p, c_int32, c_void_p, c_void_p]),
+    "fcb_stream_reset": (c_int32, [c_void_p]),
+    "fcb_stream_destroy": (None, [c_void_p]),
     "fcb_last_error": (c_char_p, [c_void_p]),
     "fcb_destroy": (None, [c_void_p]),
 }

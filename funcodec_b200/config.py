@@ -72,6 +72,32 @@ class CodecConfig:
             return self.stft_hop * (n_frames * int(math.prod(self.ratios)) - 1)
         return n_frames * self.hop_length
 
+    def stream_history(self):
+        """(history rows p, input rows per codec frame) of every conv of the time-domain stack whose output row t reads input
+        rows before t (causal: the left padding, conv.py:251-253; a transposed conv reads one earlier row)."""
+        out = []
+        rows = self.hop_length
+        dil = [self.dilation_base ** j for j in range(max(self.n_residual_layers, 1))]
+        rk = self.residual_kernel_size
+        out.append((self.kernel_size - 1, rows))                      # encoder.model.0
+        for r in reversed(self.ratios):
+            out += [((rk - 1) * d, rows) for d in dil]                  # resblock first convs (the 1x1 convs read no history)
+            out.append((r, rows))                                       # downsampling conv k = 2r, stride r: (k - 1) - (r - 1)
+            rows //= r
+        out.append((self.last_kernel_size - 1, rows))                 # final encoder conv
+        out.append((self.kernel_size - 1, rows))                      # decoder.model.0
+        for r in self.ratios:
+            out.append((1, rows))                                       # transposed conv
+            rows *= r
+            out += [((rk - 1) * d, rows) for d in dil]
+        out.append((self.last_kernel_size - 1, rows))                 # final decoder conv
+        return [(p, n) for p, n in out if p > 0]
+
+    def stream_min_first_frames(self) -> int:
+        """Frames the first chunk of a stream needs: every conv must see at least p + 1 input rows, so that its reflect
+        padding reads rows of the chunk as it does inside the whole clip."""
+        return max(1, max(-(-(p + 1) // n) for p, n in self.stream_history()))
+
     def bandwidth_per_quantizer(self) -> float:
         """ResidualVectorQuantizer.get_bandwidth_per_quantizer (funcodec/modules/quantization/vq.py:114-117)."""
         return math.log2(self.codebook_size) * self.sample_rate / self.hop_length
@@ -129,6 +155,9 @@ PRESETS: Dict[str, CodecConfig] = {
     # weight_norm with the SLSTM kept, non-causal (every norm / sequence-model combination shares the same kernels)
     "weightnorm_lstm_small": CodecConfig(name="weightnorm_lstm_small", ratios=(5, 4, 2), n_filters=8, dimension=32,
                                          codebook_size=64, num_quantizers=8, norm="weight_norm"),
+    # weight_norm, causal, with the SLSTM: the topology of Meta's causal Encodec, at the small shapes of weightnorm_lstm_small
+    "causal_lstm_small": CodecConfig(name="causal_lstm_small", ratios=(5, 4, 2), n_filters=8, dimension=32,
+                                     codebook_size=64, num_quantizers=8, norm="weight_norm", causal=True),
     "small_ds320": CodecConfig(name="small_ds320", ratios=(8, 5, 4, 2), n_filters=8, dimension=64,
                                codebook_size=256, num_quantizers=8),
 }

@@ -129,6 +129,22 @@ struct fcb_handle {
     int top_channels() const { return cfg.n_filters << cfg.n_ratios; }
 };
 
+// Chunked inference of a causal time-domain stack (DESIGN.md "Streaming").  A causal conv's output row t reads input rows
+// t - p .. t, so a chunk differs from the same rows inside the whole clip only through its p left rows: the stream keeps, per
+// conv and input source, the last p raw input rows it has seen (the history), and per SLSTM layer the final (h, c).  The
+// first chunk runs the whole-clip code unchanged (it is the start of the clip, reflect padding included) and records them;
+// later chunks read [history || chunk] without left padding.  All state is allocated at creation.
+struct fcb_stream {
+    fcb_handle* h = nullptr;
+    int kind = 0;                                  // FCB_STREAM_ENCODE / FCB_STREAM_DECODE
+    int B = 0;
+    bool started = false;                          // a first chunk has been pushed since creation / reset
+    float* mem = nullptr;                          // the one device allocation holding everything below
+    float* scale = nullptr;                        // [B] per-clip scale, or nullptr (audio_normalize off)
+    std::map<const void*, float*> hist;            // ConvW -> [2 sources][B][p][C_in]
+    std::map<const void*, float*> lstm;            // LstmW -> [layers][h | c][B][H]
+};
+
 namespace {
 
 #define FCB_CK(call)                                                                              \
@@ -425,6 +441,7 @@ struct Run {
     int B;
     cudaStream_t st;
     int phase = -1;
+    fcb_stream* s = nullptr;   // chunk of a stream: convs and SLSTM layers carry the stream's state
     std::vector<void*> live;
     Run(fcb_handle* h_, int B_, cudaStream_t st_) : h(h_), B(B_), st(st_) {}
     Run(const Run&) = delete;
@@ -489,11 +506,52 @@ InView view_of(const Act& a) {
 // One SConv1d / SConvTranspose1d / 1x1 GEMM.  in1 may be null.  want_norm=false -> plain output (LSTM input
 // projection).  Dispatch: tensor-core implicit GEMM (conv_tc.cu) when the layer has a TC weight image and the
 // input needs no division prologue, else the fp32 SIMT kernel (conv_simt.cu).
-int run_conv(Run& r, const Act& in0, const Act* in1, bool elu, const float* div_scale, const ConvW& L,
+// Rows of input history a causal conv needs: its left padding (padding_total; a transposed conv is a 2-tap conv with one
+// leading row).
+int history_rows(const ConvW& L) { return L.transposed ? 1 : (L.k - 1) * L.d - (L.s - 1); }
+
+// Streaming (Run::s set): records the last history_rows(L) raw rows of every input source.  On a stream's first chunk the conv
+// then runs as usual; on a later one *x0 / *x1 are replaced by pool tensors holding [history || chunk] and *hist_rows is set,
+// and the conv reads them without left padding.  Enqueued before the conv, hence before the caller releases the inputs.
+int stream_input(Run& r, const ConvW& L, Act* x0, Act* x1, int* hist_rows) {
+    fcb_handle* h = r.h;
+    *hist_rows = 0;
+    auto it = r.s->hist.find(&L);
+    if (it == r.s->hist.end()) return FCB_OK;
+    const int p = history_rows(L), T = x0->T, C = x0->C;
+    StreamHistParams q{};
+    q.nsrc = x1 ? 2 : 1; q.T = T; q.C = C; q.p = p;
+    Act* src[2] = {x0, x1};
+    Act tmp[2];
+    for (int i = 0; i < q.nsrc; ++i) {
+        q.x[i] = src[i]->p; q.x_stride[i] = src[i]->clip_stride; q.x_row_off[i] = src[i]->row_off;
+        q.hist[i] = it->second + (size_t)i * r.B * p * C;
+        if (src[i]->stats) return fail(h, FCB_E_INVALID, "internal: streamed input with deferred normalisation");
+        if (r.s->started) {
+            FCB_TRY(alloc_f(r, &tmp[i].p, (size_t)r.B * (p + T) * C));
+            tmp[i].owned = true; tmp[i].T = p + T; tmp[i].C = C; tmp[i].clip_stride = (long long)(p + T) * C;
+            q.tmp[i] = tmp[i].p;
+        }
+    }
+    FCB_CK(launch_stream_history(q, r.B, r.st));
+    h->launches++;
+    if (r.s->started) {
+        *x0 = tmp[0];
+        if (x1) *x1 = tmp[1];
+        *hist_rows = p;
+    }
+    return FCB_OK;
+}
+
+int run_conv(Run& r, const Act& in0_, const Act* in1_, bool elu, const float* div_scale, const ConvW& L,
              bool want_norm, Act* out) {
     fcb_handle* h = r.h;
     want_norm = want_norm && L.gamma != nullptr;   // norm: weight_norm / none -> the conv output is the layer output
     const bool causal = h->cfg.causal != 0;
+    Act in0 = in0_, in1v = in1_ ? *in1_ : Act();
+    const Act* in1 = in1_ ? &in1v : nullptr;
+    int hist_rows = 0;     // > 0: the input starts with this many rows of stream history, so there is no left padding
+    if (r.s) FCB_TRY(stream_input(r, L, &in0, in1 ? &in1v : nullptr, &hist_rows));
     ConvParams p{};
     p.in0 = view_of(in0);
     if (in1) p.in1 = view_of(*in1); else p.in1.x = nullptr;
@@ -502,7 +560,19 @@ int run_conv(Run& r, const Act& in0, const Act* in1, bool elu, const float* div_
     p.T_in = in0.T; p.C_in = in0.C;
     if (in0.C != L.cin) return fail(h, FCB_E_INVALID, "internal: channel mismatch");
     Act o;
-    if (!L.transposed) {
+    if (hist_rows > 0 && !L.transposed) {
+        // [history || chunk]: hist_rows == padding_total rows lead, and a hop-multiple chunk needs no extra right padding
+        p.K = L.k; p.S = L.s; p.D = L.d; p.pad_l = 0; p.pad_zero = 0; p.T_ext = in0.T;
+        p.T_out = (in0.T - ((L.k - 1) * L.d + 1)) / L.s + 1;
+        p.C_out = L.cout;
+        o.T = p.T_out; o.C = L.cout; o.clip_stride = (long long)p.T_out * L.cout; o.row_off = 0;
+    } else if (hist_rows > 0) {
+        // the history row stands in for the zero row ahead of the chunk; the trailing output row is the causal trim
+        p.K = 2; p.S = 1; p.D = 1; p.pad_l = 0; p.pad_zero = 1; p.T_ext = in0.T;
+        p.T_out = in0.T - 1;
+        p.C_out = L.s * L.cout;
+        o.T = p.T_out * L.s; o.C = L.cout; o.clip_stride = (long long)p.T_out * p.C_out; o.row_off = 0;
+    } else if (!L.transposed) {
         const int k = L.k, s = L.s, d = L.d;
         const int padding_total = (k - 1) * d - (s - 1);
         // get_extra_padding_for_conv1d (conv.py:57-64), integer form of ceil((T - k + pt)/s)
@@ -565,6 +635,10 @@ int run_conv(Run& r, const Act& in0, const Act* in1, bool elu, const float* div_
         }
         FCB_TRY(pool_free(r, partials));
     }
+    if (hist_rows > 0) {
+        FCB_TRY(release(r, in0));
+        if (in1) FCB_TRY(release(r, in1v));
+    }
     *out = o;
     return FCB_OK;
 }
@@ -578,6 +652,12 @@ int run_lstm(Run& r, const Act& x, const LstmW& W, Act* out) {
     Act cur = x;       // not owned copy semantics: only release what we allocate
     cur.owned = false;
     Act y;
+    float* state = nullptr;     // streaming: [layers][h | c][B][H], carried from the previous chunk after the first
+    if (r.s) {
+        auto it = r.s->lstm.find(&W);
+        if (it == r.s->lstm.end()) return fail(h, FCB_E_INVALID, "internal: no stream state for an lstm");
+        state = it->second;
+    }
     for (int l = 0; l < W.layers; ++l) {
         Act gx;
         FCB_TRY(run_conv(r, cur, nullptr, false, nullptr, W.ih[l], false, &gx));
@@ -598,8 +678,17 @@ int run_lstm(Run& r, const Act& x, const LstmW& W, Act* out) {
         sp.whh_scale = W.whh_scale[l];
         sp.whh_inv_scale = 1.0f / (W.whh_scale[l] * 4096.0f);
         sp.B = B; sp.T = T; sp.H = H;
+        float* hst = state ? state + (size_t)l * 2 * B * H : nullptr;
+        if (state) {
+            sp.h0 = r.s->started ? hst : nullptr;
+            sp.c0 = r.s->started ? hst + (size_t)B * H : nullptr;
+            sp.c_T = hst + (size_t)B * H;
+        }
         FCB_CK(launch_lstm_seq(sp, r.st));
         h->launches += 1;
+        if (state)       // h_T = the last row of h_seq (after the kernel that read h0, in stream order)
+            FCB_CK(cudaMemcpy2DAsync(hst, (size_t)H * sizeof(float), hs.p + (size_t)(T - 1) * H, (size_t)T * H * sizeof(float),
+                                     (size_t)H * sizeof(float), B, cudaMemcpyDeviceToDevice, r.st));
         FCB_TRY(release(r, gx));
         if (l > 0) FCB_TRY(release(r, cur));
         cur = hs;
@@ -628,7 +717,9 @@ int run_encoder(Run& r, const float* wav, int L, float* scale_out, Act* out) {
     FCB_TRY(phase_begin(r, FCB_PHASE_ENCODER_CONV));
     float* scale = nullptr;
     bool scale_owned = false;
-    if (h->cfg.audio_normalize) {
+    if (r.s) {
+        scale = r.s->scale;       // a stream cannot see the whole clip: it divides by the scale it was opened with
+    } else if (h->cfg.audio_normalize) {
         double* partials = nullptr;
         int nparts = sumsq_num_parts(L), np2 = 0;
         FCB_TRY(pool_alloc(r, (void**)&partials, (size_t)B * nparts * 2 * sizeof(double)));
@@ -1251,6 +1342,8 @@ int check_ready(fcb_handle* h) {
     return FCB_OK;
 }
 
+int run_rvq(Run& r, Act& f, int n_q, int64_t* codes, float* quant, float* sub_quants, float* encoder_out);
+
 int do_encode(fcb_handle* h, const float* wav, int B, int L, int n_q, int64_t* codes, float* quant, float* scale,
               float* sub_quants, float* encoder_out, cudaStream_t st) {
     if (!wav || !codes || B <= 0 || L <= 0) return fail(h, FCB_E_INVALID, "fcb_encode: bad arguments");
@@ -1260,6 +1353,14 @@ int do_encode(fcb_handle* h, const float* wav, int B, int L, int n_q, int64_t* c
     Act f;
     if (h->cfg.arch == 1) FCB_TRY(run_encoder_freq(r, wav, L, scale, &f));
     else FCB_TRY(run_encoder(r, wav, L, scale, &f));
+    return run_rvq(r, f, n_q, codes, quant, sub_quants, encoder_out);
+}
+
+// The residual vector quantizer on the encoder output f (released here).
+int run_rvq(Run& r, Act& f, int n_q, int64_t* codes, float* quant, float* sub_quants, float* encoder_out) {
+    fcb_handle* h = r.h;
+    const int B = r.B;
+    cudaStream_t st = r.st;
     FCB_TRY(phase_begin(r, FCB_PHASE_RVQ));
     RvqParams q{};
     q.in = view_of(f);
@@ -1285,6 +1386,57 @@ int do_encode(fcb_handle* h, const float* wav, int B, int L, int n_q, int64_t* c
     }
     FCB_TRY(release(r, f));
     FCB_TRY(phase_end(r));
+    return FCB_OK;
+}
+
+// The convs of a time-domain stack that read earlier rows (history_rows > 0), with the input rows per codec frame each sees.
+struct StreamLayer { const ConvW* w; int rows; bool enc; };
+std::vector<StreamLayer> stream_layers(const fcb_handle* h) {
+    std::vector<StreamLayer> v;
+    bool enc = true;
+    auto add = [&](const ConvW& w, int rows) { if (history_rows(w) > 0) v.push_back({&w, rows, enc}); };
+    const int nres = (int)(h->enc_rb.size() / h->enc_down.size());
+    int rows = h->hop();
+    add(h->enc_conv0, rows);
+    for (size_t i = 0; i < h->enc_down.size(); ++i) {
+        for (int j = 0; j < nres; ++j) {
+            const ResBlockW& rb = h->enc_rb[i * nres + j];
+            add(rb.c1, rows); add(rb.c2, rows); add(rb.sc, rows);
+        }
+        add(h->enc_down[i], rows);
+        rows /= h->enc_down[i].s;
+    }
+    add(h->enc_final, rows);
+    enc = false;
+    add(h->dec_conv0, rows);
+    for (size_t i = 0; i < h->dec_up.size(); ++i) {
+        add(h->dec_up[i], rows);
+        rows *= h->dec_up[i].s;
+        for (int j = 0; j < nres; ++j) {
+            const ResBlockW& rb = h->dec_rb[i * nres + j];
+            add(rb.c1, rows); add(rb.c2, rows); add(rb.sc, rows);
+        }
+    }
+    add(h->dec_final, rows);
+    return v;
+}
+
+// Frames the first chunk needs so that every conv sees at least p + 1 input rows: its reflect padding then reads rows
+// 1 .. p of the chunk, as it does inside the whole clip.
+int min_first_frames(const fcb_handle* h) {
+    int f = 1;
+    for (const StreamLayer& l : stream_layers(h)) {
+        const int need = (history_rows(*l.w) + 1 + l.rows - 1) / l.rows;
+        if (need > f) f = need;
+    }
+    return f;
+}
+
+int stream_check(fcb_stream* s, int frames) {
+    fcb_handle* h = s->h;
+    if (!s->started && frames < min_first_frames(h))
+        return fail(h, FCB_E_INVALID, "the first chunk of a stream needs at least " + std::to_string(min_first_frames(h)) +
+                    " frames (every conv must see more input rows than its left padding); got " + std::to_string(frames));
     return FCB_OK;
 }
 
@@ -1763,6 +1915,129 @@ int fcb_check_errors(fcb_handle* h, void* stream) {
         return fail(h, FCB_E_INVALID, "token index out of range [0, codebook_size) in fcb_decode_codes (the reference's F.embedding raises here)");
     }
     return FCB_OK;
+}
+
+int fcb_stream_min_first_frames(fcb_handle* h) {
+    FCB_TRY(check_ready(h));
+    if (h->cfg.arch != 0) return fail(h, FCB_E_INVALID, "streaming supports the time-domain Encodec only");
+    return min_first_frames(h);
+}
+
+int fcb_stream_create(fcb_handle* h, int32_t kind, int32_t B, const float* scale, fcb_stream** out) {
+    FCB_TRY(check_ready(h));
+    if (!out || (kind != FCB_STREAM_ENCODE && kind != FCB_STREAM_DECODE) || B <= 0)
+        return fail(h, FCB_E_INVALID, "fcb_stream_create: bad arguments");
+    *out = nullptr;
+    const fcb_config& c = h->cfg;
+    if (c.arch != 0)
+        return fail(h, FCB_E_INVALID, "streaming supports the time-domain Encodec only (FreqCodec's STFT frames and GroupNorm "
+                    "statistics span the whole clip)");
+    if (!c.causal)
+        return fail(h, FCB_E_INVALID, "streaming needs a causal model (causal: true): a non-causal conv reads rows after the current one");
+    if (c.norm == 0)
+        return fail(h, FCB_E_INVALID, "streaming needs norm weight_norm or none: time_group_norm normalises over the whole clip");
+    if (B > 512) return fail(h, FCB_E_INVALID, "fcb_stream_create: at most 512 clips per stream");
+    if (c.audio_normalize && !scale)
+        return fail(h, FCB_E_INVALID, "audio_normalize is set: a stream needs the per-clip scale [B] (the whole-clip path divides "
+                    "by the RMS of the whole clip, which a stream cannot know)");
+    const bool enc = kind == FCB_STREAM_ENCODE;
+    // every part starts on a 256-byte boundary (the SLSTM kernel bulk-copies h0 rows, which needs 16-byte alignment)
+    auto part = [](size_t floats) { return (floats + 63) & ~(size_t)63; };
+    size_t total = c.audio_normalize ? part(B) : 0;
+    const std::vector<StreamLayer> layers = stream_layers(h);
+    for (const StreamLayer& l : layers)
+        if (l.enc == enc) total += part((size_t)2 * B * history_rows(*l.w) * l.w->cin);
+    const LstmW& lw = enc ? h->enc_lstm : h->dec_lstm;
+    if (c.lstm_layers > 0) total += part((size_t)lw.layers * 2 * B * lw.H);
+    float* mem = nullptr;
+    FCB_CK(cudaMalloc((void**)&mem, (total ? total : 1) * sizeof(float)));
+    fcb_stream* s = new (std::nothrow) fcb_stream();
+    if (!s) { cudaFree(mem); return FCB_E_NOMEM; }
+    s->h = h; s->kind = kind; s->B = B; s->mem = mem;
+    float* cur = mem;
+    if (c.audio_normalize) {
+        s->scale = cur;
+        cur += part(B);
+        if (cudaMemcpy(s->scale, scale, (size_t)B * sizeof(float), cudaMemcpyDefault) != cudaSuccess) {
+            cudaFree(mem);
+            delete s;
+            return fail(h, FCB_E_CUDA, "fcb_stream_create: cannot read scale");
+        }
+    }
+    for (const StreamLayer& l : layers)
+        if (l.enc == enc) { s->hist[l.w] = cur; cur += part((size_t)2 * B * history_rows(*l.w) * l.w->cin); }
+    if (c.lstm_layers > 0) s->lstm[&lw] = cur;
+    *out = s;
+    return FCB_OK;
+}
+
+int fcb_stream_encode(fcb_stream* s, const float* wav, int32_t L, int32_t n_q, int64_t* codes, float* quant, void* stream) {
+    if (!s) return FCB_E_INVALID;
+    fcb_handle* h = s->h;
+    FCB_TRY(check_ready(h));
+    if (s->kind != FCB_STREAM_ENCODE) return fail(h, FCB_E_INVALID, "fcb_stream_encode: this is a decode stream");
+    if (!wav || !codes || L <= 0) return fail(h, FCB_E_INVALID, "fcb_stream_encode: bad arguments");
+    if (n_q <= 0 || n_q > h->cfg.num_quantizers) return fail(h, FCB_E_INVALID, "fcb_stream_encode: n_q out of range");
+    const int hop = h->hop();
+    if (L % hop != 0)
+        return fail(h, FCB_E_INVALID, "fcb_stream_encode: a chunk of " + std::to_string(L) + " samples is not a multiple of the hop (" +
+                    std::to_string(hop) + " samples); a partial final frame is not supported");
+    FCB_TRY(stream_check(s, L / hop));
+    Run r{h, s->B, (cudaStream_t)stream};
+    r.s = s;
+    Act f;
+    FCB_TRY(run_encoder(r, wav, L, nullptr, &f));
+    FCB_TRY(run_rvq(r, f, n_q, codes, quant, nullptr, nullptr));
+    s->started = true;
+    return FCB_OK;
+}
+
+int fcb_stream_decode_emb(fcb_stream* s, const float* emb, int32_t n_frames, float* wav_out, void* stream) {
+    if (!s) return FCB_E_INVALID;
+    fcb_handle* h = s->h;
+    FCB_TRY(check_ready(h));
+    if (s->kind != FCB_STREAM_DECODE) return fail(h, FCB_E_INVALID, "fcb_stream_decode_emb: this is an encode stream");
+    if (!emb || !wav_out || n_frames <= 0) return fail(h, FCB_E_INVALID, "fcb_stream_decode_emb: bad arguments");
+    FCB_TRY(stream_check(s, n_frames));
+    Run r{h, s->B, (cudaStream_t)stream};
+    r.s = s;
+    FCB_TRY(run_decoder_time(r, emb, n_frames, s->scale, wav_out, n_frames * h->hop()));
+    s->started = true;
+    return FCB_OK;
+}
+
+int fcb_stream_decode_codes(fcb_stream* s, const int64_t* codes, int32_t n_frames, int32_t n_q, float* wav_out, void* stream) {
+    if (!s) return FCB_E_INVALID;
+    fcb_handle* h = s->h;
+    FCB_TRY(check_ready(h));
+    if (s->kind != FCB_STREAM_DECODE) return fail(h, FCB_E_INVALID, "fcb_stream_decode_codes: this is an encode stream");
+    if (!codes || !wav_out || n_frames <= 0) return fail(h, FCB_E_INVALID, "fcb_stream_decode_codes: bad arguments");
+    if (n_q <= 0 || n_q > h->cfg.num_quantizers) return fail(h, FCB_E_INVALID, "fcb_stream_decode_codes: n_q out of range");
+    FCB_TRY(stream_check(s, n_frames));
+    cudaStream_t st = (cudaStream_t)stream;
+    Run r{h, s->B, st};
+    r.s = s;
+    float* emb = nullptr;
+    FCB_TRY(alloc_f(r, &emb, (size_t)s->B * n_frames * h->cfg.dimension));
+    FCB_CK(launch_embed_sum(reinterpret_cast<const long long*>(codes), 0, h->embed, s->B, n_frames, n_q, h->cfg.codebook_size,
+                            h->cfg.dimension, emb, h->err_flag, st));
+    h->launches++;
+    FCB_TRY(run_decoder_time(r, emb, n_frames, s->scale, wav_out, n_frames * h->hop()));
+    FCB_TRY(pool_free(r, emb));
+    s->started = true;
+    return FCB_OK;
+}
+
+int fcb_stream_reset(fcb_stream* s) {
+    if (!s) return FCB_E_INVALID;
+    s->started = false;         // the next chunk is a first chunk again: it writes every history before anything reads one
+    return FCB_OK;
+}
+
+void fcb_stream_destroy(fcb_stream* s) {
+    if (!s) return;
+    cudaFree(s->mem);
+    delete s;
 }
 
 int64_t fcb_launch_count(const fcb_handle* h) { return h ? h->launches : -1; }

@@ -61,6 +61,12 @@ struct LstmSeqParams {
     int fast_cell;        // hardware ex2 / rcp gates instead of expf / tanhf (set by the launcher: default 1, FCB_LSTM_FASTCELL=0 disables)
     float whh_scale, whh_inv_scale;   // tensor-core gate GEMM: power-of-two operand scale of W_hh and 1 / (whh_scale * 4096) (0: fp32 path)
     unsigned long long* trace;   // PROFILING ONLY (env FCB_LSTM_TRACE): [LSTM_TRACE_ITEMS][8] %globaltimer stamps of CTA 0, or nullptr
+    // carried state (streaming, engine.cu fcb_stream): h0 / c0 [B][H] initial state or nullptr (zero state: the t = 0 items skip
+    // the recurrent term); c_T [B][H] or nullptr receives the final cell state and may alias c0 (a CTA reads and writes only its
+    // own units).  h_T is row T - 1 of h_seq.
+    const float* h0;
+    const float* c0;
+    float* c_T;
 };
 constexpr int LSTM_TRACE_ITEMS = 64, LSTM_TRACE_FIRST_STEP = 100;
 cudaError_t launch_lstm_seq(const LstmSeqParams& p, cudaStream_t st);
@@ -103,5 +109,16 @@ struct OlaParams {
     float* out;                        // [B][out_len]
 };
 cudaError_t launch_overlap_add(const OlaParams& p, cudaStream_t st);
+// Streaming history of one conv's input sources (engine.cu fcb_stream): per clip and source, tmp = [hist (p rows) || x (T rows)]
+// and then hist = the last p rows of tmp; tmp == nullptr (a stream's first chunk, T >= p): hist = the last p rows of x.
+struct StreamHistParams {
+    const float* x[2];        // raw [B][rows][C] chunk input (in0, in1)
+    long long x_stride[2];    // elements between clips
+    int x_row_off[2];         // first logical row
+    float* hist[2];           // [B][p][C]
+    float* tmp[2];            // [B][p + T][C] or nullptr
+    int nsrc, T, C, p;
+};
+cudaError_t launch_stream_history(const StreamHistParams& q, int B, cudaStream_t st);
 
 }  // namespace fcb

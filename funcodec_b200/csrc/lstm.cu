@@ -84,7 +84,9 @@ constexpr float LSTM_H_SCALE = 4096.0f;   // |h| < 1: fp16 operand scale of the 
 // lo*hi + hi*lo + hi*hi in fp32, exact inverse scale afterwards): ~2^-22 relative like the fp32 FMA chain it replaces, at a
 // third of the shared-memory instruction count -- the item then costs one pass over the 128 KB W_hh slice (LDS-bound).
 // The W slice lives in shared memory in FRAGMENT ORDER: [k-step (16 k)][m-tile (16 columns)][hi | lo][lane][8 halfs].
-template <int UNITS, int GB, bool MMA>
+// CARRY: the carried-state variant (h0 / c0 / c_T of LstmSeqParams, streaming); the whole-clip launches use CARRY = false,
+// which compiles to the kernel without those branches.
+template <int UNITS, int GB, bool MMA, bool CARRY>
 __global__ void __launch_bounds__(LSTM_THREADS, 1) lstm_seq_kernel(const LstmSeqParams p, const int nbuf, const int npair, const int pload, const int nset) {
     constexpr int COLS = 4 * UNITS;            // gate columns owned by this CTA
     constexpr int KS_PER_WARP = 32 / UNITS;    // K slices inside a warp
@@ -109,6 +111,9 @@ __global__ void __launch_bounds__(LSTM_THREADS, 1) lstm_seq_kernel(const LstmSeq
     const int j0 = blockIdx.x * UNITS;
     const int n_items = T * ng;
     const unsigned nctas = gridDim.x;
+    // items that run the recurrent term are i >= i0 (the t == 0 items only with a carried h0); n = i - i0 numbers them for the
+    // h ring and the exchange buffers
+    const int i0 = (CARRY && p.h0) ? 0 : ng;
 
     // W_hh slice in the float2-paired layout: for every pair of consecutive k and every unit u two 16-byte records
     //   rec(kp, half, u) = { W[k][u][2*half], W[k+1][u][2*half], W[k][u][2*half+1], W[k+1][u][2*half+1] }
@@ -135,7 +140,10 @@ __global__ void __launch_bounds__(LSTM_THREADS, 1) lstm_seq_kernel(const LstmSeq
         const int dst = (((k >> 1) * 2 + (g >> 1)) * UNITS + uu) * 4 + ((g & 1) * 2 + (k & 1));
         Ws[dst] = __ldg(p.whh + (long long)k * 4 * H + (long long)j0 * 4 + c);
     }
-    for (int e = tid; e < ng * GB * UNITS; e += LSTM_THREADS) cS[e] = 0.f;
+    for (int e = tid; e < ng * GB * UNITS; e += LSTM_THREADS) {
+        const int b = e / UNITS;
+        cS[e] = (CARRY && p.c0 && b < B) ? p.c0[(long long)b * H + j0 + (e - b * UNITS)] : 0.f;
+    }
     if (tid == 0) {
         for (int i = 0; i < nbuf; ++i) { tc::mbar_init(hs_full + i, 1); tc::mbar_init(hs_empty + i, WS); }
         for (int i = 0; i < LSTM_PAIRS_MAX; ++i) { tc::mbar_init(red_full + i, WS); tc::mbar_init(red_empty + i, 64); }
@@ -148,8 +156,8 @@ __global__ void __launch_bounds__(LSTM_THREADS, 1) lstm_seq_kernel(const LstmSeq
         const int u = lane % UNITS, ks = lane / UNITS;
         const int set = warp / WS, wset = warp - set * WS;
         const int slice = wset * KS_PER_WARP + ks;
-        for (int i = ng + set; i < n_items; i += nset) {        // items with t == 0 need no recurrent term
-            const int n = i - ng;
+        for (int i = i0 + set; i < n_items; i += nset) {        // items with t == 0 need no recurrent term unless h0 is given
+            const int n = i - i0;
             const int hb = n % nbuf, rb = n % npair;
             tc::mbar_wait(hs_full + hb, (uint32_t)((n / nbuf) & 1));
             if (tid == 0) LSTM_TRACE(i, 2);
@@ -300,7 +308,7 @@ __global__ void __launch_bounds__(LSTM_THREADS, 1) lstm_seq_kernel(const LstmSeq
         };
         // items of this pair: those whose exchange buffer (i - ng) % npair == pair; the t == 0 items (i < ng) use no buffer and are
         // spread the same way
-        const int first = (pair + ng) % npair;                        // smallest i >= 0 with (i - ng) % npair == pair
+        const int first = (pair + i0) % npair;                        // smallest i >= 0 with (i - i0) % npair == pair
         float4 gxv = load_gx(first);
         float skv = load_skip(first);
         for (int i = first; i < n_items; i += npair) {
@@ -311,8 +319,8 @@ __global__ void __launch_bounds__(LSTM_THREADS, 1) lstm_seq_kernel(const LstmSeq
             const float4 gx_next = load_gx(i + npair);           // in flight while this item is reduced
             const float sk_next = load_skip(i + npair);
             float g4[4] = {gxv.x, gxv.y, gxv.z, gxv.w};
-            if (t > 0) {
-                const int n = i - ng, rb = pair;                 // == n % npair by construction
+            if (CARRY ? i >= i0 : t > 0) {
+                const int n = i - i0, rb = pair;                 // == n % npair by construction
                 tc::mbar_wait_backoff(red_full + rb, (uint32_t)((n / npair) & 1), 64);
                 if (ftid == 0) LSTM_TRACE(i, 5);
                 if (mine) {
@@ -337,6 +345,7 @@ __global__ void __launch_bounds__(LSTM_THREADS, 1) lstm_seq_kernel(const LstmSeq
                 float* cp = cS + (g * GB + fbb) * UNITS + fu;
                 const float c = fg * (*cp) + ig * gg;
                 *cp = c;
+                if (CARRY && p.c_T && t == T - 1) p.c_T[(long long)b * H + j] = c;
                 h = og * (p.fast_cell ? tanh_fast(c) : tanhf(c));
                 o = ((long long)b * T + t) * H + j;
                 __stcg(p.h_seq + o, h);
@@ -368,8 +377,9 @@ __global__ void __launch_bounds__(LSTM_THREADS, 1) lstm_seq_kernel(const LstmSeq
                 const int g = lane, b0 = g * GB;
                 const int nb = min(GB, B - b0);
                 float* dst = Hs + g * GB * H;
-                for (int t = 1; t < T; ++t) {
-                    tc::mbar_wait_backoff(hs_empty + g, (uint32_t)((t - 1) & 1) ^ 1, 64);
+                const int t0 = (CARRY && p.h0) ? 0 : 1;
+                for (int t = t0; t < T; ++t) {
+                    tc::mbar_wait_backoff(hs_empty + g, (uint32_t)((t - t0) & 1) ^ 1, 64);
                     if (lane == 0) LSTM_TRACE(t * ng, 0);
                     unsigned seen = ld_acquire_u32(p.barrier + g);
                     while (seen < (unsigned)t * nctas) seen = ld_acquire_u32(p.barrier + g);
@@ -377,13 +387,14 @@ __global__ void __launch_bounds__(LSTM_THREADS, 1) lstm_seq_kernel(const LstmSeq
                     asm volatile("fence.proxy.async;" ::: "memory");     // acquired generic writes -> visible to the bulk copy
                     tc::mbar_arrive_expect_tx(hs_full + g, (uint32_t)(nb * H * 4));
                     for (int bb = 0; bb < nb; ++bb)
-                        tc::bulk_g2s(dst + bb * H, p.h_seq + ((long long)(b0 + bb) * T + (t - 1)) * H, (uint32_t)(H * 4), hs_full + g);
+                        tc::bulk_g2s(dst + bb * H, (CARRY && t == 0) ? p.h0 + (long long)(b0 + bb) * H : p.h_seq + ((long long)(b0 + bb) * T + (t - 1)) * H,
+                                     (uint32_t)(H * 4), hs_full + g);
                 }
             }
         } else if (lane == 0) {
-            for (int i = ng; i < n_items; ++i) {
+            for (int i = i0; i < n_items; ++i) {
                 const int t = i / ng, g = i - t * ng;
-                const int n = i - ng, hb = n % nbuf;
+                const int n = i - i0, hb = n % nbuf;
                 const int b0 = g * GB;
                 const int nb = min(GB, B - b0);
                 tc::mbar_wait_backoff(hs_empty + hb, (uint32_t)((n / nbuf) & 1) ^ 1, 64);
@@ -395,7 +406,8 @@ __global__ void __launch_bounds__(LSTM_THREADS, 1) lstm_seq_kernel(const LstmSeq
                 tc::mbar_arrive_expect_tx(hs_full + hb, (uint32_t)(nb * H * 4));
                 float* dst = Hs + hb * GB * H;
                 for (int bb = 0; bb < nb; ++bb)
-                    tc::bulk_g2s(dst + bb * H, p.h_seq + ((long long)(b0 + bb) * T + (t - 1)) * H, (uint32_t)(H * 4), hs_full + hb);
+                    tc::bulk_g2s(dst + bb * H, (CARRY && t == 0) ? p.h0 + (long long)(b0 + bb) * H : p.h_seq + ((long long)(b0 + bb) * T + (t - 1)) * H,
+                                 (uint32_t)(H * 4), hs_full + hb);
             }
         }
     }
@@ -450,7 +462,8 @@ static cudaError_t launch_seq(const LstmSeqParams& p, cudaStream_t st) {
     const size_t smem = lstm_seq_smem_bytes(p.H, p.B, UNITS, GB, nbuf, npair);
     // the tensor-core gate GEMM needs whole k-steps per warp
     if (MMA && (p.H % 16 != 0 || ((p.H / 16) % (8 / nset)) != 0 || (p.H / 16) / (8 / nset) > 8)) return launch_seq<UNITS, GB, false>(p, st);
-    auto kern = lstm_seq_kernel<UNITS, GB, MMA>;
+    const bool carry = p.h0 || p.c0 || p.c_T;
+    auto kern = carry ? lstm_seq_kernel<UNITS, GB, MMA, true> : lstm_seq_kernel<UNITS, GB, MMA, false>;
     {
         cudaError_t e = ensure_dynamic_smem((const void*)kern, 225 * 1024);
         if (e != cudaSuccess) return e;

@@ -110,4 +110,27 @@ cudaError_t launch_fill(float* p, float v, long long n, cudaStream_t st) {
     return cudaGetLastError();
 }
 
+// One CTA per (clip, input source): the tail copy reads rows of tmp this CTA wrote, so a __syncthreads orders it, and the
+// history is overwritten only after every one of its rows has been read.
+__global__ void stream_history_kernel(const StreamHistParams q) {
+    const int b = blockIdx.x, s = blockIdx.y;
+    const int p = q.p, T = q.T, C = q.C;
+    const float* x = q.x[s] + (long long)b * q.x_stride[s] + (long long)q.x_row_off[s] * C;
+    float* hist = q.hist[s] + (long long)b * p * C;
+    if (q.tmp[s]) {
+        float* t = q.tmp[s] + (long long)b * (p + T) * C;
+        for (int i = threadIdx.x; i < p * C; i += blockDim.x) t[i] = hist[i];
+        for (long long i = threadIdx.x; i < (long long)T * C; i += blockDim.x) t[(long long)p * C + i] = x[i];
+        __syncthreads();
+        for (int i = threadIdx.x; i < p * C; i += blockDim.x) hist[i] = t[(long long)T * C + i];
+    } else {
+        for (int i = threadIdx.x; i < p * C; i += blockDim.x) hist[i] = x[(long long)(T - p) * C + i];
+    }
+}
+
+cudaError_t launch_stream_history(const StreamHistParams& q, int B, cudaStream_t st) {
+    stream_history_kernel<<<dim3(B, q.nsrc), 256, 0, st>>>(q);
+    return cudaGetLastError();
+}
+
 }  // namespace fcb

@@ -301,6 +301,17 @@ class B200Encodec:
                                                   self._stream()), "fcb_decode_emb")
         return dict(recon_speech=recon, code_indices=None, code_embeddings=[(emb, None)], sub_quants=None)
 
+    # ------------------------------------------------------------------ chunked streaming (causal models)
+    def encode_stream(self, batch_size: int, scale: Optional[torch.Tensor] = None) -> "EncodeStream":
+        """A stream that encodes B live signals chunk by chunk with the same codes as the whole clip (fcb_stream_*).  `scale`
+        [B] (or [B, 1]) is required under audio_normalize: the scale the whole-clip encode returns in code_embeddings."""
+        return EncodeStream(self, batch_size, scale)
+
+    def decode_stream(self, batch_size: int, scale: Optional[torch.Tensor] = None) -> "DecodeStream":
+        """A stream that decodes codes or quantized embeddings chunk by chunk with the same waveform as the whole clip;
+        `scale` as for encode_stream (the output is multiplied by it)."""
+        return DecodeStream(self, batch_size, scale)
+
     # ------------------------------------------------------------------ host-buffer end-to-end call (bench e2e)
     @torch.no_grad()
     def roundtrip_host(self, wav_pinned: torch.Tensor, codes_pinned: torch.Tensor, recon_pinned: torch.Tensor,
@@ -314,3 +325,99 @@ class B200Encodec:
             self._ck(self._lib.fcb_roundtrip_host(self._h, _ptr(wav_pinned), B, L, n_q, int(use_scale),
                                                   _ptr(codes_pinned), _ptr(recon_pinned), self._stream()),
                      "fcb_roundtrip_host")
+
+
+class _Stream:
+    """State of one chunked stream (include/funcodec_b200.h, "Streaming"): every chunk is a whole number of codec frames, the
+    first (after creation or reset()) at least `min_first_frames` of them."""
+
+    def __init__(self, model: B200Encodec, kind: int, batch_size: int, scale: Optional[torch.Tensor]):
+        if model.segment_dur is not None:
+            raise _capi.FcbError("streaming is not available with segment_dur: segments are encoded independently and "
+                                 "cross-faded, which a stream of chunks does not reproduce")
+        self._m = model                 # keeps the handle alive for as long as the stream
+        self.batch_size = batch_size
+        sc = None
+        if scale is not None:
+            sc = torch.as_tensor(scale).to(model.device, torch.float32).reshape(-1).contiguous()
+            if sc.numel() != batch_size:
+                raise ValueError(f"scale has {sc.numel()} entries for a batch of {batch_size}")
+        self._s = ctypes.c_void_p()
+        with torch.cuda.device(model.device):
+            model._ck(model._lib.fcb_stream_create(model._h, kind, batch_size, _ptr(sc), ctypes.byref(self._s)),
+                      "fcb_stream_create")
+        self.min_first_frames = model._ck(model._lib.fcb_stream_min_first_frames(model._h), "fcb_stream_min_first_frames")
+
+    def reset(self) -> None:
+        """Start over: the next chunk is a first chunk."""
+        self._m._ck(self._m._lib.fcb_stream_reset(self._s), "fcb_stream_reset")
+
+    def close(self) -> None:
+        if getattr(self, "_s", None):
+            self._m._lib.fcb_stream_destroy(self._s)
+            self._s = None
+
+    def __del__(self):
+        self.close()
+
+    def _check_batch(self, n: int) -> None:
+        if n != self.batch_size:
+            raise ValueError(f"chunk has {n} clips; the stream was opened for {self.batch_size}")
+
+
+class EncodeStream(_Stream):
+    def __init__(self, model: B200Encodec, batch_size: int, scale: Optional[torch.Tensor] = None):
+        super().__init__(model, _capi.FCB_STREAM_ENCODE, batch_size, scale)
+
+    @torch.no_grad()
+    def push(self, wav: torch.Tensor, n_q: Optional[int] = None):
+        """wav [B, L_c] (or [B, 1, L_c]), L_c a multiple of the hop -> (codes [n_q, B, L_c / hop] int64, the layout of
+        inference_encoding, and quantized embeddings [B, L_c / hop, D])."""
+        m = self._m
+        x = m._prep_speech(wav)
+        B, L = x.shape
+        self._check_batch(B)
+        n_q = m.cfg.num_quantizers if n_q is None else n_q
+        F = L // m.cfg.hop_length
+        codes = torch.empty((n_q, B, F), dtype=torch.int64, device=m.device)
+        quant = torch.empty((B, F, m.cfg.dimension), dtype=torch.float32, device=m.device)
+        with torch.cuda.device(m.device):
+            m._ck(m._lib.fcb_stream_encode(self._s, _ptr(x), L, n_q, _ptr(codes), _ptr(quant), m._stream()),
+                  "fcb_stream_encode")
+        return codes, quant
+
+
+class DecodeStream(_Stream):
+    def __init__(self, model: B200Encodec, batch_size: int, scale: Optional[torch.Tensor] = None):
+        super().__init__(model, _capi.FCB_STREAM_DECODE, batch_size, scale)
+
+    @torch.no_grad()
+    def push_codes(self, codes: torch.Tensor) -> torch.Tensor:
+        """codes [B, F, n_q] int64 (the layout of inference_decoding) -> waveform [B, 1, F * hop].  Synchronises to check the
+        tokens: an out-of-range one raises IndexError like inference_decoding."""
+        m = self._m
+        if codes.dim() != 3:
+            raise ValueError("codes must be [B, F, n_q]")
+        tok = codes.to(m.device, torch.int64).contiguous()
+        B, F, n_q = tok.shape
+        self._check_batch(B)
+        out = torch.empty((B, 1, F * m.cfg.hop_length), dtype=torch.float32, device=m.device)
+        with torch.cuda.device(m.device):
+            m._ck(m._lib.fcb_stream_decode_codes(self._s, _ptr(tok), F, n_q, _ptr(out), m._stream()), "fcb_stream_decode_codes")
+            if m._lib.fcb_check_errors(m._h, m._stream()) < 0:
+                raise IndexError(m._lib.fcb_last_error(m._h).decode())
+        return out
+
+    @torch.no_grad()
+    def push_emb(self, emb: torch.Tensor) -> torch.Tensor:
+        """emb [B, F, D] quantized embeddings (LauraTTS-style vocoding) -> waveform [B, 1, F * hop]."""
+        m = self._m
+        if emb.dim() != 3 or emb.shape[-1] != m.cfg.dimension:
+            raise ValueError("emb must be [B, F, D]")
+        e = emb.to(m.device, torch.float32).contiguous()
+        B, F, _ = e.shape
+        self._check_batch(B)
+        out = torch.empty((B, 1, F * m.cfg.hop_length), dtype=torch.float32, device=m.device)
+        with torch.cuda.device(m.device):
+            m._ck(m._lib.fcb_stream_decode_emb(self._s, _ptr(e), F, _ptr(out), m._stream()), "fcb_stream_decode_emb")
+        return out

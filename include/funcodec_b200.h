@@ -183,6 +183,38 @@ FCB_API int fcb_roundtrip_segmented(fcb_handle* h, const float* wav, int32_t B, 
                                     int32_t n_q, int32_t use_scale, int64_t* codes, float* quant, float* scale,
                                     float* recon, void* stream);
 
+/* ---- Streaming (causal time-domain models: causal = 1, norm weight_norm / none, arch 0).  A stream codes a live signal chunk by
+ * chunk and gives the same bits as the whole clip through fcb_encode / fcb_decode_*: a causal conv's output row t reads input
+ * rows t - p .. t only, so the stream keeps the last p input rows of every conv (and the final (h, c) of every SLSTM layer) and
+ * feeds them to the next chunk in place of the left padding.  Its state lives in device memory allocated at creation:
+ * sum over the convs of 2 * p * C_in * B floats, plus 2 * layers * B * H for the SLSTM.
+ *   - chunks are whole codec frames (a multiple of the hop in samples); a partial final frame is refused;
+ *   - the first chunk (after creation or fcb_stream_reset) needs at least fcb_stream_min_first_frames(h) frames: there every
+ *     conv pads by reflection like the whole clip does, which needs more input rows than its padding;
+ *   - audio_normalize: the whole-clip path divides by the RMS of the whole clip, which a stream cannot know, so the per-clip
+ *     `scale` dev [B] (e.g. the one fcb_encode returns) is required at creation; the encoder divides by it and the decoder
+ *     multiplies by it.  Without audio_normalize the scale is 1 and `scale` is ignored.  Copied synchronously;
+ *   - n_q may change from chunk to chunk (the quantizer keeps no state).  Calls are asynchronous on `stream` like every other
+ *     call; streams of one handle share no state, but like the handle's other calls they must be issued on one CUDA stream.
+ *     After a failed call, reset the stream.  Destroy streams before their handle.
+ * Refused with a message: non-causal models, time_group_norm, FreqCodec (arch 1). */
+#define FCB_STREAM_ENCODE 0
+#define FCB_STREAM_DECODE 1
+typedef struct fcb_stream fcb_stream;
+FCB_API int fcb_stream_min_first_frames(fcb_handle* h);
+FCB_API int fcb_stream_create(fcb_handle* h, int32_t kind, int32_t B, const float* scale, fcb_stream** out);
+/* wav dev [B, L] with L a multiple of the hop; codes dev [n_q, B, L / hop] int64; quant dev [B, L / hop, D] or NULL. */
+FCB_API int fcb_stream_encode(fcb_stream* s, const float* wav, int32_t L, int32_t n_q, int64_t* codes, float* quant,
+                              void* stream);
+/* codes dev [B, n_frames, n_q] int64 (out-of-range tokens raise the fcb_check_errors flag); wav_out dev [B, n_frames * hop]. */
+FCB_API int fcb_stream_decode_codes(fcb_stream* s, const int64_t* codes, int32_t n_frames, int32_t n_q, float* wav_out,
+                                    void* stream);
+/* emb dev [B, n_frames, D] quantized embeddings; wav_out dev [B, n_frames * hop]. */
+FCB_API int fcb_stream_decode_emb(fcb_stream* s, const float* emb, int32_t n_frames, float* wav_out, void* stream);
+/* Start over: the next chunk is a first chunk. */
+FCB_API int fcb_stream_reset(fcb_stream* s);
+FCB_API void fcb_stream_destroy(fcb_stream* s);
+
 /* Number of kernels this handle has launched since creation (bench.py's gpu_launches). */
 FCB_API int64_t fcb_launch_count(const fcb_handle* h);
 /* Enable/disable per-phase device timing (CUDA events on `stream`); phase ids FCB_PHASE_*. */

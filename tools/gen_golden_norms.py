@@ -11,3 +11,4 @@ from gen_golden import model_case  # noqa: E402
 if __name__ == "__main__":
     model_case("soundstream_causal_small", 3, 3, 40 * 21 + 9, 41, bit_widths=(None,))
     model_case("weightnorm_lstm_small", 4, 2, 40 * 25 + 3, 42, bit_widths=(None, 8000))
+    model_case("causal_lstm_small", 6, 2, 40 * 25, 43, bit_widths=(None,))      # {weight_norm, causal, SLSTM}
